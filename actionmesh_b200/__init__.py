@@ -1,4 +1,4 @@
-"""actionmesh_b200 — B200-native (sm_100a) Stage-I denoising hot path of ActionMesh behind the reference's own seams.
+"""actionmesh_b200 — H100-native (sm_90a) Stage-I denoising hot path of ActionMesh behind the reference's own seams.
 
 Host code is Python/PyTorch plumbing; all arithmetic runs in hand-written CUDA kernels loaded through a C ABI
 (include/actionmesh_b200.h).  There is no CPU fallback: importing the package is cheap, but every op raises if

@@ -10,12 +10,12 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libactionmesh_b200.so")
 
-ABI_VERSION = 13
+ABI_VERSION = 14
 
 EXPORTS = [
     "amb_last_error", "amb_abi_version", "amb_device_info", "amb_cfg_euler_step", "amb_layernorm",
     "amb_cast_f32_bf16", "amb_patchify", "amb_timestep_embedding", "amb_alpha_rows", "amb_point_embedding",
-    "amb_displacement_out", "amb_split3_bf16", "amb_softmax_split3", "amb_resize_h_u8", "amb_resize_v_normalize", "amb_alpha_stats", "amb_composite_crop_pad", "amb_nearest_neighbors", "amb_add_bias_rows", "amb_gemm_bf16", "amb_flash_attn_fwd", "amb_attn_small_f32", "amb_debug_set_attn_trace",
+    "amb_displacement_out", "amb_split3_bf16", "amb_softmax_split3", "amb_resize_h_u8", "amb_resize_v_normalize", "amb_alpha_stats", "amb_composite_crop_pad", "amb_nearest_neighbors", "amb_add_bias_rows", "amb_gemm_bf16", "amb_flash_attn_fwd", "amb_attn_small_f32",
 ]
 
 
@@ -67,7 +67,7 @@ def load_library() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise AmbError(
-            f"{LIB_PATH} not found: the sm_100a CUDA extension has not been built. "
+            f"{LIB_PATH} not found: the sm_90a CUDA extension has not been built. "
             "Run `python __graft_entry__.py` (there is no CPU fallback)."
         )
     lib = C.CDLL(LIB_PATH)
@@ -103,7 +103,6 @@ def load_library() -> C.CDLL:
     lib.amb_add_bias_rows.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]
     lib.amb_gemm_bf16.argtypes = [C.POINTER(GemmArgs), C.c_void_p]
     lib.amb_flash_attn_fwd.argtypes = [C.POINTER(AttnArgs), C.c_void_p]
-    lib.amb_debug_set_attn_trace.argtypes = [C.c_void_p]
     lib.amb_attn_small_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_float,
                                        C.c_void_p, C.c_int64, C.c_void_p]
     for name in EXPORTS:

@@ -2,8 +2,8 @@
 
 Same call signature as `AttentionProcessor.__call__` (actionmesh/model/utils/attention_processor.py:36-46).  It reads the
 diffusers `Attention` container it is attached to (`to_q/to_k/to_v/to_out[0]/norm_q/norm_k/heads/is_cross_attention`)
-and runs the whole processor body on the sm_100a kernels: fused-QKV tcgen05 GEMM whose epilogue does the
-head-interleaved split (folded into a one-time weight permutation), RMS qk-norm and RoPE; tcgen05 flash attention;
+and runs the whole processor body on the sm_90a kernels: fused-QKV wgmma GEMM whose epilogue does the
+head-interleaved split (folded into a one-time weight permutation), RMS qk-norm and RoPE; wgmma flash attention;
 to_out GEMM with bias.  Returns a NEW tensor of the input dtype and never aliases the (normed) input, as the block
 relies on (`hidden_states + self.s_attn(self.norm_s_attn(hidden_states))`, block.py:137).
 

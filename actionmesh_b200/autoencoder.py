@@ -1,4 +1,4 @@
-"""B200-native Stage-II temporal autoencoder — drop-in for `ActionMeshAutoencoder`
+"""H100-native Stage-II temporal autoencoder — drop-in for `ActionMeshAutoencoder`
 (actionmesh/model/temporal_autoencoder.py:30-269), the first "next" row of SURVEY 8(f).
 
 Same duck type the pipeline uses (pipeline.py:186-199,358-372): `forward(latent, framestep, source_alpha, target_alphas,
@@ -9,14 +9,14 @@ Two precision regimes, as in the reference:
   * the 16-block self-attention trunk over the T*(N+1) latent+alpha tokens runs under autocast in the reference with an
     fp32 residual stream (`cat([bf16 latents, fp32 alpha])` promotes, temporal_autoencoder.py:256) and bf16 GEMMs/SDPA.
     Here: h fp32, LayerNorm fp32 -> bf16, fused QKV GEMM (head split folded in the weights, RoPE in the epilogue, no
-    q/k norm), the tcgen05 flash attention, to_out/FF GEMMs with fp32 residual epilogues.  Tokens are laid out
+    q/k norm), the wgmma flash attention, to_out/FF GEMMs with fp32 residual epilogues.  Tokens are laid out
     frame-major [N latents | 1 alpha token] per frame instead of the reference's [T*N latents | T alpha tokens]; every
     op of the block is token-local or permutation invariant (unmasked attention), and a token's RoPE position is its
     frame in both layouts, so results are identical and the denoiser's kernels are reused unchanged.
   * the final vertex-query cross-attention block runs with autocast DISABLED (fp32) in the reference
     (temporal_autoencoder.py:264-266).  Here it runs on the bf16 tensor cores at fp32-grade accuracy: every operand is
     split x = hi + lo and concatenated along K (ops.split3), attention is evaluated unfused per head as
-    S = Q'K'^T (fp32) -> row softmax (fp32, ops.softmax_split3) -> O = P'V'^T, all with fp32 accumulation in TMEM.
+    S = Q'K'^T (fp32) -> row softmax (fp32, ops.softmax_split3) -> O = P'V'^T, all with fp32 accumulation.
 There is no torch arithmetic on the path (torch owns buffers and does two memcpy-style `copy_`s) and no CPU fallback.
 """
 from __future__ import annotations
@@ -91,7 +91,7 @@ class B200Autoencoder:
     def to(self, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise AmbError("B200Autoencoder only runs on a CUDA (sm_100) device; there is no CPU path")
+            raise AmbError("B200Autoencoder only runs on a CUDA (sm_90) device; there is no CPU path")
         if self._loaded and device != self._device:
             self._w = {k: v.to(device) for k, v in self._w.items()}
         self._device = device

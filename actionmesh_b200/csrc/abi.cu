@@ -87,10 +87,10 @@ int ensure_smem_optin_impl(const void* kern, int bytes) {
 int num_sms() {
   static int n[16] = {};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev < 16 && n[dev]) return n[dev];
   int v = 0;
-  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 148;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
   if (dev < 16) n[dev] = v;
   return v;
 }

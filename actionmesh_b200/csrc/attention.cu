@@ -1,705 +1,236 @@
-// tcgen05 flash-attention forward for sm_100a (non-causal, no mask):  O = softmax(scale · Q Kᵀ) V
+// wgmma flash-attention forward for sm_90a (non-causal, no mask):  O = softmax(scale · Q Kᵀ) V
+// Replaces F.scaled_dot_product_attention at actionmesh/model/utils/attention_processor.py:133-139 (head_dim 128) and
+// DinoV2's attention (head_dim 64).
 //
-// One CTA owns 256 query rows of one (batch, head): two 128-row tiles ping-ponged through one tensor pipe.
-//   warp 0      TMA producer: Q tiles once, then a STAGES-deep ring of 64-key K/V tiles (strided 4-D tensor maps, so
-//               q/k/v are read in place from the fused QKV GEMM output)
-//   warp 1      MMA issuer (one lane):  S_i = Q_i·K_jᵀ   (SS, 128x64x16, K-major K tile)
-//                                       O_i += P_i·V_j   (SS, 128xDx16, MN-major V tile; P_i staged as bf16 in smem)
-//   warps 2-5   softmax warpgroup for tile 0;  warps 6-9: tile 1.   thread == query row (tcgen05.ld 32x32b), so the row
-//               max / row sum need no cross-thread traffic.  exp2 with the scale folded in; O is rescaled lazily (only
-//               when the running max grew by more than 2^8), which is exact after the final 1/rowsum normalisation.
-// TMEM: S0 [0,64) S1 [64,128) O0 [128,128+D) O1 [128+D,128+2D)  -> 512 columns allocated.
-// The issue order  S0 S1 | PV0 S0' PV1 S1' | ...  keeps the tensor pipe busy with tile 1 while warpgroup 0 is in softmax.
-#include <type_traits>
+// One CTA owns 128 query rows of one (batch, head); three warpgroups:
+//   warpgroup 0     TMA producer: the Q tile once, then a STAGES-deep ring of 128-key K and V tiles (strided 4-D / 5-D tensor
+//                   maps, so q/k/v are read in place from the fused QKV GEMM output; K and V on separate barriers so that
+//                   Q·Kᵀ starts before V has landed)
+//   warpgroups 1-2  consumers, 64 query rows each:  S = Q·Kᵀ (wgmma, both operands in shared memory) -> online softmax in
+//                   registers (exp2 with the scale folded in; a row lives in one quad, so its max / sum are two shuffles) ->
+//                   O += P·V (wgmma with P as the register A operand, V MN-major from shared memory).  The two consumer
+//                   warpgroups interleave: one computes exponentials while the other's MMAs run.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "attention.cuh"
 
 namespace amb {
 
-// debug: timeline buffer set through amb_debug_set_attn_trace (never on the product path unless set)
-static long long* g_attn_trace = nullptr;
-constexpr int TRACE_J0 = 100, TRACE_NJ = 16, TRACE_EV = 8;  // iterations [100,116), 8 event slots per (role, iteration)
-__device__ __forceinline__ void trace_ev(long long* tr, int role, int j, int ev) {
-  if (tr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && j >= TRACE_J0 && j < TRACE_J0 + TRACE_NJ)
-    tr[(role * TRACE_NJ + (j - TRACE_J0)) * TRACE_EV + ev] = clock64();
-}
+constexpr int ATT_BQ = 128;   // query rows per CTA (64 per consumer warpgroup)
+constexpr int ATT_BK = 128;   // keys per K/V tile
+constexpr int ATT_THREADS = 384;
+constexpr int ATT_STAGES = 2;
 
-constexpr int ATT_BQ = 128;   // rows per query tile
-constexpr int ATT_BK = 64;    // keys per K/V tile
-constexpr int ATT_THREADS = 320;
-
-template <int D, int STAGES>
+template <int D>
 struct AttnSmem {
-  static constexpr int Q_TILE_BYTES = ATT_BQ * D * 2;          // one query tile (D/64 column halves of 16 KB)
-  static constexpr int KV_TILE_BYTES = ATT_BK * D * 2;         // one K or V tile
-  static constexpr int P_TILE_BYTES = ATT_BQ * ATT_BK * 2;     // 16 KB
+  static constexpr int BOX_BYTES = 128 * 128;                   // 128 rows x 64 columns of bf16 (one SWIZZLE_128B box)
+  static constexpr int Q_BYTES = (D / 64) * BOX_BYTES;
+  static constexpr int KV_BYTES = (D / 64) * BOX_BYTES;         // one K or V tile of 128 keys
   static constexpr int Q_OFF = 0;
-  static constexpr int P_OFF = 2 * Q_TILE_BYTES;
-  static constexpr int KV_OFF = P_OFF + 2 * P_TILE_BYTES;
-  static constexpr int BAR_OFF = KV_OFF + STAGES * 2 * KV_TILE_BYTES;
-  static constexpr int NUM_BARS = 1 + 2 * STAGES + 2 + 2 + 2;  // q_full, kv_full[], kv_empty[], s_full[2], p_ready[2], o_full[2]
-  static constexpr int TOTAL = BAR_OFF + NUM_BARS * 8 + 16 + 1024;
+  static constexpr int K_OFF = Q_BYTES;
+  static constexpr int V_OFF = K_OFF + ATT_STAGES * KV_BYTES;
+  static constexpr int BAR_OFF = V_OFF + ATT_STAGES * KV_BYTES;
+  static constexpr int NUM_BARS = 1 + 3 * ATT_STAGES;            // q_full, k_full[], v_full[], kv_empty[]
+  static constexpr int TOTAL = BAR_OFF + NUM_BARS * 8 + 1024;
 };
 
-template <int D, int STAGES>
+template <int D>
+__device__ __forceinline__ void pv_k16(float* o, const uint32_t* a, uint64_t vdesc) {
+  if constexpr (D == 128) wgmma_rs_n128_tb(o, a, vdesc, 1u);
+  else wgmma_rs_n64_tb(o, a, vdesc, 1u);
+}
+
+template <int D>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                       const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
-  using L = AttnSmem<D, STAGES>;
-  constexpr int DH = D / 64;  // 64-column halves per row
+  using L = AttnSmem<D>;
+  constexpr int DH = D / 64;  // 64-column boxes per row
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
-  uint64_t* kv_full = q_full + 1;
-  uint64_t* kv_empty = kv_full + STAGES;
-  uint64_t* s_full = kv_empty + STAGES;  // [2]
-  uint64_t* p_ready = s_full + 2;        // [2]
-  uint64_t* o_full = p_ready + 2;        // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 2);
+  uint64_t* k_full = q_full + 1;
+  uint64_t* v_full = k_full + ATT_STAGES;
+  uint64_t* kv_empty = v_full + ATT_STAGES;
 
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);  // provably warp-uniform (uniform datapath for role code)
+  const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);  // warp-uniform role
+  const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * (2 * ATT_BQ);
+  const int q0 = blockIdx.x * ATT_BQ;
   const int head = blockIdx.y;
   const int batch = blockIdx.z;
-  const int n_kv = p.kv_chunks * ((p.sk_chunk + ATT_BK - 1) / ATT_BK);  // K/V tiles in total
   const int tiles_per_chunk = (p.sk_chunk + ATT_BK - 1) / ATT_BK;
+  const int n_kv = p.kv_chunks * tiles_per_chunk;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      mbar_init(q_full, 1);
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(&kv_full[s], 1);
-        mbar_init(&kv_empty[s], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&s_full[i], 1);
-        mbar_init(&p_ready[i], 128);
-        mbar_init(&o_full[i], 1);
-      }
-      fence_mbar_init();
+    mbar_init(q_full, 1);
+    for (int s = 0; s < ATT_STAGES; ++s) {
+      mbar_init(&k_full[s], 1);
+      mbar_init(&v_full[s], 1);
+      mbar_init(&kv_empty[s], 8);  // one arrival per consumer warp
     }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
+    fence_mbar_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    // ===================== TMA producer (warp converged, one elected lane issues) =====================
-    if (elect_one()) {
-      mbar_expect_tx(q_full, 2 * L::Q_TILE_BYTES);
-      for (int i = 0; i < 2; ++i)
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    reg_dealloc<24>();
+    if (warp == 0) {
+      if (elect_one()) {
+        mbar_expect_tx(q_full, L::Q_BYTES);
         for (int c = 0; c < DH; ++c)
-          tma_load_4d(smem + L::Q_OFF + i * L::Q_TILE_BYTES + c * (ATT_BQ * 128), &tmQ, q_full, c * 64,
-                      q0 + i * ATT_BQ, head, batch, kEvictFirst);
-    }
-    __syncwarp();
-    int s = 0;
-    uint32_t phase = 0;
-    for (int j = 0; j < n_kv; ++j) {
-      const int chunk = j / tiles_per_chunk;
-      const int key0 = (j - chunk * tiles_per_chunk) * ATT_BK;
-      mbar_wait(&kv_empty[s], phase ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&kv_full[s], 2 * L::KV_TILE_BYTES);
-        uint8_t* sk = smem + L::KV_OFF + s * 2 * L::KV_TILE_BYTES;
-        uint8_t* sv = sk + L::KV_TILE_BYTES;
-        for (int c = 0; c < DH; ++c) {  // K/V maps are 5-D: (d, key, head, batch, chunk)
-          tma_load_5d(sk + c * (ATT_BK * 128), &tmK, &kv_full[s], c * 64, key0, head, batch, chunk, kEvictLast);
-          tma_load_5d(sv + c * (ATT_BK * 128), &tmV, &kv_full[s], c * 64, key0, head, batch, chunk, kEvictLast);
+          tma_load_4d(smem + L::Q_OFF + c * L::BOX_BYTES, &tmQ, q_full, c * 64, q0, head, batch, kEvictFirst);
+      }
+      __syncwarp();
+      int s = 0;
+      uint32_t phase = 0;
+      for (int j = 0; j < n_kv; ++j) {
+        const int chunk = j / tiles_per_chunk;
+        const int key0 = (j - chunk * tiles_per_chunk) * ATT_BK;
+        mbar_wait(&kv_empty[s], phase ^ 1);
+        if (elect_one()) {  // K/V maps are 5-D: (d, key, head, batch, chunk)
+          uint8_t* sk = smem + L::K_OFF + s * L::KV_BYTES;
+          uint8_t* sv = smem + L::V_OFF + s * L::KV_BYTES;
+          mbar_expect_tx(&k_full[s], L::KV_BYTES);
+          for (int c = 0; c < DH; ++c)
+            tma_load_5d(sk + c * L::BOX_BYTES, &tmK, &k_full[s], c * 64, key0, head, batch, chunk, kEvictLast);
+          mbar_expect_tx(&v_full[s], L::KV_BYTES);
+          for (int c = 0; c < DH; ++c)
+            tma_load_5d(sv + c * L::BOX_BYTES, &tmV, &v_full[s], c * 64, key0, head, batch, chunk, kEvictLast);
         }
+        __syncwarp();
+        if (++s == ATT_STAGES) { s = 0; phase ^= 1; }
       }
-      __syncwarp();
-      if (++s == STAGES) { s = 0; phase ^= 1; }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (warp converged; descriptors stay in uniform registers) =====================
-    constexpr uint32_t idesc_qk = make_idesc_bf16(ATT_BQ, ATT_BK, 0, 0);  // S[128 x 64]  = Q (K-major) · K (K-major)
-    constexpr uint32_t idesc_pv = make_idesc_bf16(ATT_BQ, D, 0, 1);      // O[128 x D]  += P (K-major) · V (MN-major)
-    const uint32_t sq_addr = smem_u32(smem + L::Q_OFF);
-    const uint32_t sp_addr = smem_u32(smem + L::P_OFF);
-    const uint32_t skv_addr = smem_u32(smem + L::KV_OFF);
-    const uint32_t ts0 = tmem_base, ts1 = tmem_base + 64, to0 = tmem_base + 128, to1 = tmem_base + 128 + D;
-
-    auto issue_qk = [=](int i, int stage) {
-      const uint64_t qd = make_desc_kmajor_sw128(sq_addr + i * L::Q_TILE_BYTES);
-      const uint64_t kd = make_desc_kmajor_sw128(skv_addr + stage * 2 * L::KV_TILE_BYTES);
-      const uint32_t d = i ? ts1 : ts0;
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < D / 16; ++k)  // descriptor address field is (bytes >> 4)
-          mma_ss(d, qd + ((k >> 2) * (ATT_BQ * 128 / 16) + (k & 3) * 2), kd + ((k >> 2) * (ATT_BK * 128 / 16) + (k & 3) * 2),
-                 idesc_qk, k != 0);
-        tc_commit(&s_full[i]);
-      }
-      __syncwarp();
-    };
-    auto issue_pv = [=](int i, int stage, bool accumulate) {
-      const uint64_t pd = make_desc_kmajor_sw128(sp_addr + i * L::P_TILE_BYTES);
-      // V tile: [64 keys][64 d] boxes of 128-B rows; 16 keys = 2048 B; next 64 d-columns ATT_BK*128 B further
-      const uint64_t vd = make_desc_mnmajor_sw128(skv_addr + stage * 2 * L::KV_TILE_BYTES + L::KV_TILE_BYTES, ATT_BK * 128);
-      const uint32_t d = i ? to1 : to0;
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < ATT_BK / 16; ++k)
-          mma_ss(d, pd + 2 * k, vd + 128 * k, idesc_pv, (accumulate || k != 0) ? 1u : 0u);
-      }
-      __syncwarp();
-    };
-    auto commit = [=](uint64_t* bar) {
-      if (elect_one()) tc_commit(bar);
-      __syncwarp();
-    };
-
-    mbar_wait(q_full, 0);
-    mbar_wait(&kv_full[0], 0);
-    tc_fence_after();
-    issue_qk(0, 0);
-    issue_qk(1, 0);
-    int s = 0;
-    uint32_t phase = 0;
-    for (int j = 0; j < n_kv; ++j) {
-      int s_next = s + 1;
-      uint32_t phase_next = phase;
-      if (s_next == STAGES) { s_next = 0; phase_next ^= 1; }
-      const bool has_next = (j + 1 < n_kv);
-      // ---- tile 0
-      mbar_wait(&p_ready[0], j & 1);
-      tc_fence_after();
-      issue_pv(0, s, j > 0);
-      if (has_next) {
-        mbar_wait(&kv_full[s_next], phase_next);
-        tc_fence_after();
-        issue_qk(0, s_next);
-      } else {
-        commit(&o_full[0]);
-      }
-      // ---- tile 1
-      mbar_wait(&p_ready[1], j & 1);
-      tc_fence_after();
-      issue_pv(1, s, j > 0);
-      commit(&kv_empty[s]);  // K_j and V_j fully consumed once everything issued so far has completed
-      if (has_next) {
-        issue_qk(1, s_next);
-      } else {
-        commit(&o_full[1]);
-      }
-      s = s_next;
-      phase = phase_next;
     }
   } else {
-    // ===================== softmax warpgroups =====================
-    const int wg = (warp - 2) >> 2;       // 0 or 1: which query tile
-    const int quarter = warp & 3;         // TMEM lane quarter accessible to this warp
-    const uint32_t tmem_s[2] = {tmem_base, tmem_base + 64};
-    const uint32_t tmem_o[2] = {tmem_base + 128, tmem_base + 128 + D};
-    const int row_in_tile = quarter * 32 + lane;
-    const int q_row = q0 + wg * ATT_BQ + row_in_tile;
-    const uint32_t lane_sel = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t s_addr = tmem_s[wg] + lane_sel;
-    const uint32_t o_addr = tmem_o[wg] + lane_sel;
-    uint8_t* sp_row = smem + L::P_OFF + wg * L::P_TILE_BYTES + row_in_tile * 128;
-    const int sw = row_in_tile & 7;
-
-    float m_used = -INFINITY;  // max (raw score units) the stored exponentials are relative to
-    float row_sum = 0.f;
+    // ===================== consumers =====================
+    reg_alloc<240>();
+    const int q = lane & 3;
+    const int r_local = (wg - 1) * 64 + (warp & 3) * 16 + (lane >> 2);  // my rows: r_local and r_local + 8
+    const uint32_t sq_addr = smem_u32(smem + L::Q_OFF) + (wg - 1) * 64 * 128;
+    const uint32_t sk_addr = smem_u32(smem + L::K_OFF);
+    const uint32_t sv_addr = smem_u32(smem + L::V_OFF);
+    const float c = p.scale_log2;
     const int last_valid = p.sk_chunk - (tiles_per_chunk - 1) * ATT_BK;  // valid keys in the last tile of each chunk
 
+    float o[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+    float m_a = -INFINITY, m_b = -INFINITY;  // running maxima (raw score units) of my two rows
+    float l_a = 0.f, l_b = 0.f;              // partial row sums over my columns
+
+    mbar_wait(q_full, 0);
+    int s = 0, jj = 0;
+    uint32_t phase = 0;
     for (int j = 0; j < n_kv; ++j) {
-      mbar_wait(&s_full[wg], j & 1);
-      tc_fence_after();
-      float sc[ATT_BK];
-      tmem_ld_x32f(s_addr, sc);
-      tmem_ld_x32f(s_addr + 32, sc + 32);
-      tmem_wait_ld();
-      const int jj = j % tiles_per_chunk;
+      // ---- S = Q Kᵀ (64 x 128 per warpgroup)
+      float sc[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) sc[i] = 0.f;
+      mbar_wait(&k_full[s], phase);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < D / 16; ++k) {  // 16 columns of d per step: +32 B inside a 128-B row, next box after 4 steps
+        const uint32_t off = (k >> 2) * L::BOX_BYTES + (k & 3) * 32;
+        wgmma_ss_n128(sc, make_desc_kmajor_sw128(sq_addr + off), make_desc_kmajor_sw128(sk_addr + s * L::KV_BYTES + off), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < 64; ++i) reg_fence(sc[i]);
+
+      // ---- online softmax: sc[4i + {0,1}] = row a, keys 8i + 2q + {0,1}; sc[4i + {2,3}] = row b, same keys
       if (jj == tiles_per_chunk - 1 && last_valid < ATT_BK) {
 #pragma unroll
-        for (int c = 0; c < ATT_BK; ++c)
-          if (c >= last_valid) sc[c] = -INFINITY;
-      }
-      float mx = sc[0];
-#pragma unroll
-      for (int c = 1; c < ATT_BK; ++c) mx = fmaxf(mx, sc[c]);
-      const float m_new = fmaxf(m_used, mx);
-      // lazy rescale: keep the old reference max unless it is stale by more than 2^8
-      const bool need = (m_new - m_used) * p.scale_log2 > 8.0f;  // also true on the first tile (m_used = -inf)
-      if (j == 0) {
-        m_used = m_new;
-      } else if (__any_sync(0xffffffffu, need)) {
-        const float alpha = need ? ex2_approx((m_used - m_new) * p.scale_log2) : 1.0f;
-        if (need) {
-          m_used = m_new;
-          row_sum *= alpha;
+        for (int i = 0; i < 16; ++i) {
+          const int key = 8 * i + 2 * q;
+          if (key >= last_valid) sc[4 * i] = sc[4 * i + 2] = -INFINITY;
+          if (key + 1 >= last_valid) sc[4 * i + 1] = sc[4 * i + 3] = -INFINITY;
         }
-#pragma unroll 1
-        for (int c = 0; c < D; c += 32) {
-          float ov[32];
-          tmem_ld_x32f(o_addr + c, ov);
-          tmem_wait_ld();
-#pragma unroll
-          for (int t = 0; t < 32; ++t) ov[t] *= alpha;
-          tmem_st_x32f(o_addr + c, ov);
-        }
-        tmem_wait_st();
       }
-      const float mb = m_used * p.scale_log2;
-      float psum = 0.f;
+      if (++jj == tiles_per_chunk) jj = 0;
+      float mx_a = m_a, mx_b = m_b;
 #pragma unroll
-      for (int c = 0; c < ATT_BK; c += 8) {
-        float e[8];
-#pragma unroll
-        for (int t = 0; t < 8; ++t) {
-          e[t] = ex2_approx(fmaf(sc[c + t], p.scale_log2, -mb));
-          psum += e[t];
-        }
-        uint4 pk;
-        pk.x = pack_bf16(e[0], e[1]);
-        pk.y = pack_bf16(e[2], e[3]);
-        pk.z = pack_bf16(e[4], e[5]);
-        pk.w = pack_bf16(e[6], e[7]);
-        // 128B-swizzled K-major row: 16-byte chunk index XOR (row % 8)
-        *reinterpret_cast<uint4*>(sp_row + (((c >> 3) ^ sw) << 4)) = pk;
+      for (int i = 0; i < 16; ++i) {
+        mx_a = fmaxf(mx_a, fmaxf(sc[4 * i], sc[4 * i + 1]));
+        mx_b = fmaxf(mx_b, fmaxf(sc[4 * i + 2], sc[4 * i + 3]));
       }
-      row_sum += psum;
-      fence_proxy_async_smem();  // P (generic-proxy stores) -> visible to the tensor core's async-proxy reads
-      tc_fence_before();
-      mbar_arrive(&p_ready[wg]);
+      mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1));
+      mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1));
+      mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
+      mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
+      const float al_a = ex2_approx((m_a - mx_a) * c), al_b = ex2_approx((m_b - mx_b) * c);  // 0 on the first tile
+      m_a = mx_a;
+      m_b = mx_b;
+      const float mb_a = m_a * c, mb_b = m_b * c;
+      uint32_t pk[32];
+      float ts_a = 0.f, ts_b = 0.f;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const float ea0 = ex2_approx(fmaf(sc[4 * i], c, -mb_a)), ea1 = ex2_approx(fmaf(sc[4 * i + 1], c, -mb_a));
+        const float eb0 = ex2_approx(fmaf(sc[4 * i + 2], c, -mb_b)), eb1 = ex2_approx(fmaf(sc[4 * i + 3], c, -mb_b));
+        ts_a += ea0 + ea1;
+        ts_b += eb0 + eb1;
+        pk[2 * i] = pack_bf16(ea0, ea1);      // A fragment of P·V: (row a, keys 2q, 2q+1) / (row b, ...) of 8-key group i
+        pk[2 * i + 1] = pack_bf16(eb0, eb1);
+      }
+      l_a = l_a * al_a + ts_a;
+      l_b = l_b * al_b + ts_b;
+#pragma unroll
+      for (int i = 0; i < D / 8; ++i) {
+        o[4 * i] *= al_a;
+        o[4 * i + 1] *= al_a;
+        o[4 * i + 2] *= al_b;
+        o[4 * i + 3] *= al_b;
+      }
+
+      // ---- O += P V: 16 keys per step = 2048 B of the MN-major V tile; the second 64-column box of d is BOX_BYTES further
+      mbar_wait(&v_full[s], phase);
+      wgmma_fence();
+      const uint32_t vbase = sv_addr + s * L::KV_BYTES;
+#pragma unroll
+      for (int kk = 0; kk < ATT_BK / 16; ++kk)
+        pv_k16<D>(o, pk + 4 * kk, make_desc_mnmajor_sw128(vbase + kk * 2048, L::BOX_BYTES));
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < D / 2; ++i) reg_fence(o[i]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&kv_empty[s]);  // this warp is done with K_j and V_j
+      if (++s == ATT_STAGES) { s = 0; phase ^= 1; }
     }
 
     // ---- epilogue: O / rowsum -> bf16 -> global (b, s, h, d)
-    mbar_wait(&o_full[wg], 0);
-    tc_fence_after();
-    const float inv = 1.0f / row_sum;
-    __nv_bfloat16* orow = p.o + (long long)batch * p.o_stride_b + (long long)head * p.o_stride_h + (long long)q_row * p.o_stride_s;
-#pragma unroll 1
-    for (int c = 0; c < D; c += 32) {
-      float ov[32];
-      tmem_ld_x32f(o_addr + c, ov);
-      tmem_wait_ld();
-      if (q_row < p.sq) {
+    l_a += __shfl_xor_sync(0xffffffffu, l_a, 1);
+    l_b += __shfl_xor_sync(0xffffffffu, l_b, 1);
+    l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
+    l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
+    const float inv_a = 1.0f / l_a, inv_b = 1.0f / l_b;
+    const int qr_a = q0 + r_local, qr_b = qr_a + 8;
+    __nv_bfloat16* obase = p.o + (long long)batch * p.o_stride_b + (long long)head * p.o_stride_h + 2 * q;
 #pragma unroll
-        for (int t = 0; t < 32; t += 8) {
-          uint4 pk;
-          pk.x = pack_bf16(ov[t] * inv, ov[t + 1] * inv);
-          pk.y = pack_bf16(ov[t + 2] * inv, ov[t + 3] * inv);
-          pk.z = pack_bf16(ov[t + 4] * inv, ov[t + 5] * inv);
-          pk.w = pack_bf16(ov[t + 6] * inv, ov[t + 7] * inv);
-          *reinterpret_cast<uint4*>(orow + c + t) = pk;
-        }
-      }
+    for (int i = 0; i < D / 8; ++i) {
+      if (qr_a < p.sq)
+        *reinterpret_cast<uint32_t*>(obase + (long long)qr_a * p.o_stride_s + 8 * i) = pack_bf16(o[4 * i] * inv_a, o[4 * i + 1] * inv_a);
+      if (qr_b < p.sq)
+        *reinterpret_cast<uint32_t*>(obase + (long long)qr_b * p.o_stride_s + 8 * i) = pack_bf16(o[4 * i + 2] * inv_b, o[4 * i + 3] * inv_b);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
-
-constexpr int V2_BK = 128;  // keys per K/V tile of the v4 kernel
-
-// =====================================================================================================================
-// v4 (head_dim 128, the product kernel): 128-key K/V tiles, P kept in TMEM (aliasing S, consumed by a TS-form MMA), P
-// handed to the MMA warp in two halves so P·V of keys 0-63 overlaps the exponentials of keys 64-127, and TWO threads
-// per query row.  16 softmax warps: for query tile i, warps 8i..8i+3 own keys 0-63 of every 128-key tile and warps
-// 8i+4..8i+7 own keys 64-127 (a warp may only touch TMEM lanes 32*(warp%4)+[0,32), so both halves cover all 4 lane
-// quarters).  Halving the per-thread work halves the softmax latency on the critical QK -> softmax -> PV chain and gives
-// every SM sub-partition 4 softmax warps to interleave.  The two halves of a row exchange their partial row maxima
-// through shared memory (one 256-thread named barrier per tile step); partial row sums are combined once at the end.
-//   warp 16 = TMA producer, warp 17 = MMA issuer + TMEM owner.
-//   TMEM: S0 [0,128) S1 [128,256) O0 [256,384) O1 [384,512); P_i = bf16 pairs in the first 32 columns of each key-half of S_i.
-//   Tensor-pipe order:  S0 S1 | PV0a PV0b S0' | PV1a PV1b S1' | ...
-// =====================================================================================================================
-constexpr int V4_THREADS = 576;
-
-template <int KSTAGES, int VSTAGES>
-struct AttnV4Smem {
-  static constexpr int TILE_BYTES = 128 * 128 * 2;
-  static constexpr int Q_OFF = 0;
-  static constexpr int K_OFF = 2 * TILE_BYTES;
-  static constexpr int V_OFF = K_OFF + KSTAGES * TILE_BYTES;
-  static constexpr int XCH_OFF = V_OFF + VSTAGES * TILE_BYTES;          // float[2 tiles][2 halves][128 rows]
-  static constexpr int BAR_OFF = XCH_OFF + 2 * 2 * 128 * 4;
-  static constexpr int NUM_BARS = 1 + 2 * KSTAGES + 2 * VSTAGES + 2 + 2 + 2 + 2;
-  static constexpr int TOTAL = BAR_OFF + NUM_BARS * 8 + 16 + 1024;
-};
-
-template <int KSTAGES, int VSTAGES, int EMU>
-__global__ void __launch_bounds__(V4_THREADS, 1)  // 18 warps are allocated as 5 warpgroups: 96 registers per thread
-flash_attn_fwd_v4_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                         const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
-  using L = AttnV4Smem<KSTAGES, VSTAGES>;
-  constexpr int D = 128;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* xch = reinterpret_cast<float*>(smem + L::XCH_OFF);
-  uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
-  uint64_t* k_full = q_full + 1;
-  uint64_t* k_empty = k_full + KSTAGES;
-  uint64_t* v_full = k_empty + KSTAGES;
-  uint64_t* v_empty = v_full + VSTAGES;
-  uint64_t* s_full = v_empty + VSTAGES;  // [2]
-  uint64_t* p_a = s_full + 2;            // [2] keys 0-63 of P ready (arrivals: the 128 "half 0" threads)
-  uint64_t* p_b = p_a + 2;               // [2] keys 64-127 of P ready (the 128 "half 1" threads)
-  uint64_t* o_full = p_b + 2;            // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 2);
-
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
-  const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * (2 * ATT_BQ);
-  const int head = blockIdx.y;
-  const int batch = blockIdx.z;
-  const int tiles_per_chunk = (p.sk_chunk + V2_BK - 1) / V2_BK;
-  const int n_kv = p.kv_chunks * tiles_per_chunk;
-
-  if (warp == 16 && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-  }
-  if (warp == 17) {
-    if (lane == 0) {
-      mbar_init(q_full, 1);
-      for (int s = 0; s < KSTAGES; ++s) { mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 1); }
-      for (int s = 0; s < VSTAGES; ++s) { mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 1); }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&s_full[i], 1);
-        mbar_init(&p_a[i], 128);
-        mbar_init(&p_b[i], 128);
-        mbar_init(&o_full[i], 1);
-      }
-      fence_mbar_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 16) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      mbar_expect_tx(q_full, 2 * L::TILE_BYTES);
-      for (int i = 0; i < 2; ++i)
-        for (int c = 0; c < 2; ++c)
-          tma_load_4d(smem + L::Q_OFF + i * L::TILE_BYTES + c * 16384, &tmQ, q_full, c * 64, q0 + i * ATT_BQ, head,
-                      batch, kEvictFirst);
-    }
-    __syncwarp();
-    int ks = 0, vs = 0;
-    uint32_t kph = 0, vph = 0;
-    for (int j = 0; j < n_kv; ++j) {
-      const int chunk = j / tiles_per_chunk;
-      const int key0 = (j - chunk * tiles_per_chunk) * V2_BK;
-      mbar_wait(&k_empty[ks], kph ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&k_full[ks], L::TILE_BYTES);
-        uint8_t* sk = smem + L::K_OFF + ks * L::TILE_BYTES;
-        tma_load_5d(sk, &tmK, &k_full[ks], 0, key0, head, batch, chunk, kEvictLast);
-        tma_load_5d(sk + 16384, &tmK, &k_full[ks], 64, key0, head, batch, chunk, kEvictLast);
-      }
-      __syncwarp();
-      if (++ks == KSTAGES) { ks = 0; kph ^= 1; }
-      mbar_wait(&v_empty[vs], vph ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&v_full[vs], L::TILE_BYTES);
-        uint8_t* sv = smem + L::V_OFF + vs * L::TILE_BYTES;
-        tma_load_5d(sv, &tmV, &v_full[vs], 0, key0, head, batch, chunk, kEvictLast);
-        tma_load_5d(sv + 16384, &tmV, &v_full[vs], 64, key0, head, batch, chunk, kEvictLast);
-      }
-      __syncwarp();
-      if (++vs == VSTAGES) { vs = 0; vph ^= 1; }
-    }
-  } else if (warp == 17) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc_qk = make_idesc_bf16(ATT_BQ, V2_BK, 0, 0);
-    constexpr uint32_t idesc_pv = make_idesc_bf16(ATT_BQ, D, 0, 1);
-    const uint32_t sq_addr = smem_u32(smem + L::Q_OFF);
-    const uint32_t sk_addr = smem_u32(smem + L::K_OFF);
-    const uint32_t sv_addr = smem_u32(smem + L::V_OFF);
-
-    auto issue_qk = [=](int i, int kstage) {
-      const uint64_t qd = make_desc_kmajor_sw128(sq_addr + i * L::TILE_BYTES);
-      const uint64_t kd = make_desc_kmajor_sw128(sk_addr + kstage * L::TILE_BYTES);
-      const uint32_t d = tmem_base + i * 128;
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < D / 16; ++k) {
-          const uint32_t off = (k >> 2) * (16384 / 16) + (k & 3) * 2;
-          mma_ss(d, qd + off, kd + off, idesc_qk, k != 0);
-        }
-        tc_commit(&s_full[i]);
-      }
-      __syncwarp();
-    };
-    auto issue_pv_half = [=](int i, int vstage, int half, bool first_tile) {
-      const uint64_t vd = make_desc_mnmajor_sw128(sv_addr + vstage * L::TILE_BYTES, 16384);
-      const uint32_t d = tmem_base + 256 + i * 128;
-      // P of key-half h lives in the first 32 columns of THAT half's own S columns (h*64): a half's P never overwrites
-      // scores the other half's threads still have to re-read.
-      const uint32_t pa = tmem_base + i * 128 + half * 64;
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const int k = half * 4 + kk;
-          mma_ts(d, pa + kk * 8, vd + 128 * k, idesc_pv, (!first_tile || k != 0) ? 1u : 0u);
-        }
-      }
-      __syncwarp();
-    };
-    auto commit = [=](uint64_t* bar) {
-      if (elect_one()) tc_commit(bar);
-      __syncwarp();
-    };
-
-    mbar_wait(q_full, 0);
-    mbar_wait(&k_full[0], 0);
-    tc_fence_after();
-    issue_qk(0, 0);
-    issue_qk(1, 0);
-    commit(&k_empty[0]);
-    int ks = 0, vs = 0;
-    uint32_t kph = 0, vph = 0;
-    for (int j = 0; j < n_kv; ++j) {
-      int ks_next = ks + 1;
-      uint32_t kph_next = kph;
-      if (ks_next == KSTAGES) { ks_next = 0; kph_next ^= 1; }
-      const bool has_next = (j + 1 < n_kv);
-      const uint32_t par = j & 1;
-      mbar_wait(&v_full[vs], vph);
-      mbar_wait(&p_a[0], par);
-      if (lane == 0) trace_ev(p.trace, 4, j, 0);
-      tc_fence_after();
-      issue_pv_half(0, vs, 0, j == 0);
-      mbar_wait(&p_b[0], par);
-      if (lane == 0) trace_ev(p.trace, 4, j, 1);
-      tc_fence_after();
-      issue_pv_half(0, vs, 1, j == 0);
-      if (has_next) {
-        mbar_wait(&k_full[ks_next], kph_next);
-        tc_fence_after();
-        issue_qk(0, ks_next);
-      } else {
-        commit(&o_full[0]);
-      }
-      if (lane == 0) trace_ev(p.trace, 4, j, 2);
-      mbar_wait(&p_a[1], par);
-      if (lane == 0) trace_ev(p.trace, 4, j, 3);
-      tc_fence_after();
-      issue_pv_half(1, vs, 0, j == 0);
-      mbar_wait(&p_b[1], par);
-      if (lane == 0) trace_ev(p.trace, 4, j, 4);
-      tc_fence_after();
-      issue_pv_half(1, vs, 1, j == 0);
-      commit(&v_empty[vs]);
-      if (has_next) {
-        issue_qk(1, ks_next);
-        commit(&k_empty[ks_next]);
-      } else {
-        commit(&o_full[1]);
-      }
-      if (lane == 0) trace_ev(p.trace, 4, j, 5);
-      ks = ks_next;
-      kph = kph_next;
-      if (++vs == VSTAGES) { vs = 0; vph ^= 1; }
-    }
-  } else {
-    // ===================== softmax: 2 tiles x 2 key-halves x 4 lane quarters =====================
-    const int tile = warp >> 3;
-    const int half = (warp >> 2) & 1;
-    const int quarter = warp & 3;
-    const int row_in_tile = quarter * 32 + lane;
-    const int q_row = q0 + tile * ATT_BQ + row_in_tile;
-    const uint32_t lane_sel = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t s_addr = tmem_base + tile * 128 + half * 64 + lane_sel;   // my 64 score columns
-    const uint32_t p_addr = s_addr;                                          // my 32 packed-P columns alias my own scores
-    const uint32_t o_addr = tmem_base + 256 + tile * 128 + half * 64 + lane_sel;  // my 64 O columns (rescale / epilogue)
-    float* x_mine = xch + (tile * 2 + half) * 128 + row_in_tile;
-    const float* x_other = xch + (tile * 2 + (half ^ 1)) * 128 + row_in_tile;
-    uint64_t* my_p_bar = half ? &p_b[tile] : &p_a[tile];
-    const uint32_t bar_id = 1 + tile;  // named barrier of this tile's 256 softmax threads
-
-    float m_used = -INFINITY;
-    float row_sum = 0.f;  // partial: my 64 keys of every tile
-    const int last_valid = p.sk_chunk - (tiles_per_chunk - 1) * V2_BK;  // valid keys in the last tile of a chunk
-
-    auto softmax_step = [&](int j, auto masked_tag) {
-      constexpr bool MASKED = decltype(masked_tag)::value;
-      const bool tracer = (quarter == 0 && lane == 0);
-      if (tracer) trace_ev(p.trace, tile * 2 + half, j, 0);
-      mbar_wait(&s_full[tile], j & 1);
-      if (tracer) trace_ev(p.trace, tile * 2 + half, j, 1);
-      tc_fence_after();
-      // ---- pass 1: partial row max over my 64 scores (two 32-column reads; the values are re-read in pass 2 to keep
-      //      the register footprint at 32 scores: 18 warps are allocated as 5 warpgroups => 96 registers per thread)
-      float mxp;
-      {
-        float a[32], b[32];
-        tmem_ld_x32f(s_addr, a);
-        tmem_ld_x32f(s_addr + 32, b);
-        tmem_wait_ld();
-        if (MASKED) {
-#pragma unroll
-          for (int t = 0; t < 32; ++t) {
-            if (half * 64 + t >= last_valid) a[t] = -INFINITY;
-            if (half * 64 + 32 + t >= last_valid) b[t] = -INFINITY;
-          }
-        }
-        float mx0 = fmaxf(a[0], a[1]), mx1 = fmaxf(b[0], b[1]);
-#pragma unroll
-        for (int t = 2; t < 32; t += 2) {
-          mx0 = fmaxf(mx0, fmaxf(a[t], a[t + 1]));
-          mx1 = fmaxf(mx1, fmaxf(b[t], b[t + 1]));
-        }
-        mxp = fmaxf(mx0, mx1);
-      }
-      // exchange the partial row max with the thread that owns the other 64 keys of this row
-      *x_mine = mxp;
-      if (tracer) trace_ev(p.trace, tile * 2 + half, j, 2);
-      named_bar_sync(bar_id, 256);
-      if (tracer) trace_ev(p.trace, tile * 2 + half, j, 3);
-      const float m_new = fmaxf(m_used, fmaxf(mxp, *x_other));
-      const bool need = (m_new - m_used) * p.scale_log2 > 8.0f;
-      if (j == 0) {
-        m_used = m_new;
-      } else if (__any_sync(0xffffffffu, need)) {
-        // rare: rescale my 64 columns of O (both halves of a row take the same decision: same m values).  Both halves
-        // finish long before either hands over P (the exponentials follow), so P·V never meets a half-rescaled O.
-        const float alpha = need ? ex2_approx((m_used - m_new) * p.scale_log2) : 1.0f;
-        if (need) {
-          m_used = m_new;
-          row_sum *= alpha;
-        }
-#pragma unroll 1
-        for (int c = 0; c < 64; c += 32) {
-          float ov[32];
-          tmem_ld_x32f(o_addr + c, ov);
-          tmem_wait_ld();
-#pragma unroll
-          for (int t = 0; t < 32; ++t) ov[t] *= alpha;
-          tmem_st_x32f(o_addr + c, ov);
-        }
-        tmem_wait_st();
-        named_bar_sync(3 + tile * 4 + quarter, 64);  // my row-partner warp has rescaled its O columns too
-      }
-      // ---- pass 2: exponentials in four 16-score chunks; the TMEM read of chunk c+1 is issued before the math of chunk c
-      //      (software prefetch: its latency hides behind 16 exponentials); bf16 P overwrites my own consumed S columns
-      const float mb = m_used * p.scale_log2;
-      const uint64_t scale2 = pk2(p.scale_log2, p.scale_log2), nmb2 = pk2(-mb, -mb);
-      uint64_t psum2 = pk2(0.f, 0.f), psum2b = pk2(0.f, 0.f);  // two independent accumulation chains
-      float scb[2][16];
-      tmem_ld_x16f(s_addr, scb[0]);
-      tmem_wait_ld();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        if (c < 3) tmem_ld_x16f(s_addr + (c + 1) * 16, scb[(c + 1) & 1]);
-        const float* sc = scb[c & 1];
-        uint32_t pk[8];
-#pragma unroll
-        for (int t = 0; t < 16; t += 2) {
-          float x0, x1, e0, e1;
-          upk2(fma2(pk2(sc[t], sc[t + 1]), scale2, nmb2), x0, x1);
-          if (EMU > 0 && ((t >> 1) % (EMU > 0 ? EMU : 1)) == EMU - 1) {
-            exp2_poly2(x0, x1, e0, e1);
-          } else {
-            e0 = ex2_approx(x0);
-            e1 = ex2_approx(x1);
-          }
-          if (MASKED) {  // the scores were re-read unmasked: zero the tail keys explicitly
-            if (half * 64 + c * 16 + t >= last_valid) e0 = 0.f;
-            if (half * 64 + c * 16 + t + 1 >= last_valid) e1 = 0.f;
-          }
-          if ((t >> 1) & 1) psum2b = add2(psum2b, pk2(e0, e1));
-          else psum2 = add2(psum2, pk2(e0, e1));
-          pk[t >> 1] = pack_bf16(e0, e1);
-        }
-        tmem_wait_ld();                       // chunk c+1 has landed (and chunk c's columns are fully consumed)
-        tmem_st_x8(p_addr + c * 8, pk);       // P of chunk c -> columns [8c, 8c+8): always inside already-read scores
-      }
-      if (tracer) trace_ev(p.trace, tile * 2 + half, j, 4);
-      tmem_wait_st();
-      tc_fence_before();
-      mbar_arrive(my_p_bar);
-      if (tracer) trace_ev(p.trace, tile * 2 + half, j, 5);
-      {
-        float s0, s1;
-        upk2(add2(psum2, psum2b), s0, s1);
-        row_sum += s0 + s1;
-      }
-    };
-
-    const bool has_tail = last_valid < V2_BK;
-    int jj = 0;
-    for (int j = 0; j < n_kv; ++j) {
-      const bool tail = has_tail && (jj == tiles_per_chunk - 1);
-      if (++jj == tiles_per_chunk) jj = 0;
-      if (tail) softmax_step(j, std::true_type{});
-      else softmax_step(j, std::false_type{});
-    }
-
-    // ---- epilogue: combine the two partial row sums, normalise my 64 columns of O, store bf16
-    mbar_wait(&o_full[tile], 0);
-    tc_fence_after();
-    named_bar_sync(bar_id, 256);  // everyone is past the last max exchange before the buffer is reused for the sums
-    *x_mine = row_sum;
-    named_bar_sync(bar_id, 256);
-    const float inv = 1.0f / (row_sum + *x_other);
-    __nv_bfloat16* orow = p.o + (long long)batch * p.o_stride_b + (long long)head * p.o_stride_h +
-                          (long long)q_row * p.o_stride_s + half * 64;
-#pragma unroll 1
-    for (int c = 0; c < 64; c += 32) {
-      float ov[32];
-      tmem_ld_x32f(o_addr + c, ov);
-      tmem_wait_ld();
-      if (q_row < p.sq) {
-#pragma unroll
-        for (int t = 0; t < 32; t += 8) {
-          uint4 pk;
-          pk.x = pack_bf16(ov[t] * inv, ov[t + 1] * inv);
-          pk.y = pack_bf16(ov[t + 2] * inv, ov[t + 3] * inv);
-          pk.z = pack_bf16(ov[t + 4] * inv, ov[t + 5] * inv);
-          pk.w = pack_bf16(ov[t + 6] * inv, ov[t + 7] * inv);
-          *reinterpret_cast<uint4*>(orow + c + t) = pk;
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 17) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-
-template <int D, int STAGES>  // baseline single-CTA kernel (head_dim 64: DinoV2's attention)
-static int launch_attn_v1(const amb_attn_args* a, cudaStream_t stream) {
-  using L = AttnSmem<D, STAGES>;
+template <int D>
+static int launch_attn(const amb_attn_args* a, cudaStream_t stream) {
+  using L = AttnSmem<D>;
   CUtensorMap tmQ, tmK, tmV;
   int r = encode_attn_maps(a, D, ATT_BQ, ATT_BK, ATT_BK, &tmQ, &tmK, &tmV);
   if (r) return r;
-  const AttnParams p = make_attn_params(a, g_attn_trace);
-  dim3 grid((a->sq + 2 * ATT_BQ - 1) / (2 * ATT_BQ), a->heads, a->batch);
-  auto kern = flash_attn_fwd_kernel<D, STAGES>;
+  const AttnParams p = make_attn_params(a);
+  dim3 grid((a->sq + ATT_BQ - 1) / ATT_BQ, a->heads, a->batch);
+  auto kern = flash_attn_fwd_kernel<D>;
   r = ensure_smem_optin(kern, L::TOTAL);
   if (r) return r;
   kern<<<grid, ATT_THREADS, L::TOTAL, stream>>>(tmQ, tmK, tmV, p);
@@ -707,30 +238,9 @@ static int launch_attn_v1(const amb_attn_args* a, cudaStream_t stream) {
   return AMB_OK;
 }
 
-// single-CTA head_dim-128 kernel (two 128-row query tiles per CTA)
-static int launch_attn_v4(const amb_attn_args* a, cudaStream_t stream) {
-  using L4 = AttnV4Smem<2, 2>;
-  CUtensorMap tmQ, tmK, tmV;
-  int r = encode_attn_maps(a, 128, ATT_BQ, V2_BK, V2_BK, &tmQ, &tmK, &tmV);
-  if (r) return r;
-  const AttnParams p = make_attn_params(a, g_attn_trace);
-  dim3 grid((a->sq + 2 * ATT_BQ - 1) / (2 * ATT_BQ), a->heads, a->batch);
-  auto kern = flash_attn_fwd_v4_kernel<2, 2, 4>;
-  r = ensure_smem_optin(kern, L4::TOTAL);
-  if (r) return r;
-  kern<<<grid, V4_THREADS, L4::TOTAL, stream>>>(tmQ, tmK, tmV, p);
-  AMB_CHECK_CUDA(cudaGetLastError());
-  return AMB_OK;
-}
-
 }  // namespace amb
 
 using namespace amb;
-
-extern "C" int amb_debug_set_attn_trace(void* device_buffer) {
-  amb::g_attn_trace = reinterpret_cast<long long*>(device_buffer);
-  return AMB_OK;
-}
 
 extern "C" int amb_flash_attn_fwd(const amb_attn_args* a, amb_stream_t stream) {
   AMB_CHECK_ARG(a && a->q && a->k && a->v && a->o, "flash_attn: null pointer");
@@ -745,11 +255,6 @@ extern "C" int amb_flash_attn_fwd(const amb_attn_args* a, amb_stream_t stream) {
                 "flash_attn: kv_chunks * sk_chunk must equal sk");
   AMB_CHECK_ARG(a->batch <= 65535 && a->heads <= 65535, "flash_attn: grid limits");
   cudaStream_t s = (cudaStream_t)stream;
-  if (a->head_dim == 64) return launch_attn_v1<64, 4>(a, s);
-  // head_dim 128: the CTA-pair kernel for long key loops (its two softmax sets, three S buffers and the fix-up pass pay off
-  // from a few dozen key tiles on: the inflated self-attention, 257 tiles); the single-CTA kernel for short ones (the
-  // per-frame cross-attention to 257 context tokens = 3 tiles).
-  const int key_tiles = (a->sk + 127) / 128;
-  if (key_tiles < 48) return launch_attn_v4(a, s);
-  return launch_attn_pair(a, g_attn_trace, s);
+  if (a->head_dim == 64) return launch_attn<64>(a, s);
+  return launch_attn<128>(a, s);
 }

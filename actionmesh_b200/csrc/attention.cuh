@@ -1,5 +1,4 @@
-// Shared declarations of the flash-attention translation units (attention.cu: single-CTA kernels; attention_pair.cu:
-// the CTA-pair kernel).
+// Tensor maps and parameters of the flash-attention kernel (attention.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -14,8 +13,6 @@ struct AttnParams {
   int heads, sq, sk;
   int kv_chunks, sk_chunk;   // kv split into chunks along the outermost tensor-map coordinate
   float scale_log2;          // scale * log2(e)
-  long long* trace;          // optional device buffer for the clock64 timeline of CTA (0,0,0) (debug; NULL = off)
-  int* dirty;                // pair kernel: one flag per (batch, head, 256-row unit) the fast pass asks the exact pass to redo
 };
 
 // Q map is 4-D (d, s, head, batch); K/V maps are 5-D (d, key, head, batch, chunk) with free strides: one chunk per rank
@@ -46,7 +43,7 @@ inline int encode_attn_maps(const amb_attn_args* a, int D, uint32_t q_rows, uint
   return enc_kv(tmV, a->v, a->v_stride_s, a->v_stride_h, a->v_stride_b, a->v_chunk_stride, v_rows);
 }
 
-inline AttnParams make_attn_params(const amb_attn_args* a, long long* trace) {
+inline AttnParams make_attn_params(const amb_attn_args* a) {
   AttnParams p;
   p.o = reinterpret_cast<__nv_bfloat16*>(a->o);
   p.o_stride_b = a->o_stride_b; p.o_stride_h = a->o_stride_h; p.o_stride_s = a->o_stride_s;
@@ -54,12 +51,7 @@ inline AttnParams make_attn_params(const amb_attn_args* a, long long* trace) {
   p.kv_chunks = a->kv_chunks > 0 ? a->kv_chunks : 1;
   p.sk_chunk = p.kv_chunks > 1 ? a->sk_chunk : a->sk;
   p.scale_log2 = a->scale * 1.4426950408889634f;
-  p.trace = trace;
-  p.dirty = nullptr;
   return p;
 }
-
-// CTA-pair kernel (head_dim 128), attention_pair.cu
-int launch_attn_pair(const amb_attn_args* a, long long* trace, cudaStream_t stream);
 
 }  // namespace amb

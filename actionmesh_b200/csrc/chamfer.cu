@@ -3,9 +3,9 @@
 // Replaces scipy's KDTree.query at actionbench/chamfer.py:44-50 (compute_chamfer_score) and :78-82
 // (compute_motion_chamfer_score): for every query point the Euclidean distance to, and the index of, its nearest reference
 // point.  Brute force: a query per thread, reference points streamed through shared memory in tiles, the reference set split
-// over blockIdx.y so a few thousand queries still fill 148 SMs; partial results meet in one 64-bit atomicMin per query on
+// over blockIdx.y so a few thousand queries still fill 132 SMs; partial results meet in one 64-bit atomicMin per query on
 // (float bits of d^2 << 32 | index) — valid because d^2 >= 0 orders like its bit pattern, and ties resolve to the lowest
-// index.  fp32 FMA work: 10 000 x 100 000 pairs are 8 GFLOP — microseconds on a B200, where the reference's KD-tree build
+// index.  fp32 FMA work: 10 000 x 100 000 pairs are 8 GFLOP — microseconds on an H100, where the reference's KD-tree build
 // + query takes seconds on the host.
 #include "common.cuh"
 #include "../../include/actionmesh_b200.h"

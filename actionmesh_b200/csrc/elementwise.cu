@@ -1,4 +1,4 @@
-// HBM-bound elementwise / row-reduction kernels of the denoising path (sm_100a).
+// HBM-bound elementwise / row-reduction kernels of the denoising path (sm_90a).
 //  - cfg_euler_step : CFG combine + Euler flow update + observed-frame mask   (scheduler.py:238-248, guidance.py:95-118)
 //  - layernorm      : affine LayerNorm with fp32 statistics                    (block.py:64,83,98,107)
 //  - cast / timestep embedding / bias-row add
@@ -298,9 +298,9 @@ __global__ void __launch_bounds__(256) split3_kernel(const float* __restrict__ s
 
 // Row softmax of fp32 scores, written as the A-pattern split [P_hi | P_lo | P_hi] with each part n_pad wide and zeros in
 // the padding columns [n, n_pad).  One 512-thread CTA per row, two sweeps and no shared-memory staging of the row (an
-// earlier version staged the 131 KB row in shared memory, which capped occupancy at one CTA per SM = 25 % and 2.7 TB/s,
-// profiles/r01_ncu_gemm2_stage2_summary.txt): sweep 1 keeps a per-thread online (max, sum) pair, sweep 2 re-reads the row
-// (L2-resident: 4 CTAs/SM x 148 SMs x 131 KB = 78 MB) and writes exp(x - max) / sum.
+// earlier version staged the 131 KB row in shared memory, which capped occupancy at one CTA per SM): sweep 1 keeps a
+// per-thread online (max, sum) pair, sweep 2 re-reads the row (4 CTAs/SM x 132 SMs x 131 KB = 69 MB of rows in flight
+// against the 50 MB L2) and writes exp(x - max) / sum.
 __global__ void __launch_bounds__(512, 4) softmax_split3_kernel(const float* __restrict__ s, long long ld_s, int n, int n_pad,
                                                                 float scale, __nv_bfloat16* __restrict__ dst, long long ld_dst) {
   __shared__ float red_m[16], red_l[16];

@@ -1,4 +1,4 @@
-"""B200Denoiser — sm_100a implementation of ActionMesh's temporal 3D DiT denoiser behind the reference's duck type.
+"""B200Denoiser — sm_90a (H100) implementation of ActionMesh's temporal 3D DiT denoiser behind the reference's duck type.
 
 Mirrors `ActionMeshDenoiser` (reference actionmesh/model/temporal_denoiser.py:23-249): same constructor fields, same
 state-dict keys (SURVEY A.1), same `forward(hidden_states, context, framestep, diffusion_time, mask, freqs_rot)` ->
@@ -118,7 +118,7 @@ class B200Denoiser:
     def to(self, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise AmbError("B200Denoiser runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise AmbError("B200Denoiser runs on CUDA (sm_90a) only; there is no CPU fallback")
         if device.index is None:
             device = torch.device("cuda", torch.cuda.current_device())
         if self._loaded and self._device != device:

@@ -1,7 +1,7 @@
 """ClassifierFreeGuidance — same dataclass surface as the reference (actionmesh/scheduler/guidance.py:14-118).
 
 `cfg_at_inference` / `aggregate_cfg` / `get_unobserved_mask` keep the reference's generic tensor semantics so any
-duck-typed model works; the B200 fast path in `B200SchedulerFlow` never materialises the CFG batch (the branches share
+duck-typed model works; the CUDA fast path in `B200SchedulerFlow` never materialises the CFG batch (the branches share
 their latents) and fuses `aggregate_cfg` with the Euler update in one kernel (amb_cfg_euler_step).
 """
 from __future__ import annotations

@@ -3,8 +3,8 @@
 Mirrors actionmesh/model/image_encoder.py:16-55: constructor kwargs `pretrained_dino_feature_extractor`,
 `pretrained_dino_model`; `.encode_images(list[PIL]) -> (T, 257, 1024) fp32`; `.device`, `.eval()`, `.to()`.
 The transformer (HF `Dinov2Model`, transformers/models/dinov2/modeling_dinov2.py: patch-embed conv, CLS + interpolated
-position embeddings, 24 x [LN, MHA(16 heads, d_h 64), LayerScale, LN, MLP GELU, LayerScale], final LN) runs on the sm_100a
-kernels: patchify (im2col) -> tcgen05 GEMM, LayerNorm, fused-QKV tcgen05 GEMM, tcgen05 flash attention (head_dim 64),
+position embeddings, 24 x [LN, MHA(16 heads, d_h 64), LayerScale, LN, MLP GELU, LayerScale], final LN) runs on the sm_90a
+kernels: patchify (im2col) -> wgmma GEMM, LayerNorm, fused-QKV wgmma GEMM, wgmma flash attention (head_dim 64),
 GEMM epilogues with bias / GELU / LayerScale / fp32 residual.
 
 Precision.  The reference runs DinoV2 in fp32, outside autocast (pipeline.py:664-667), so the default here is fp32-grade
@@ -12,7 +12,7 @@ Precision.  The reference runs DinoV2 in fp32, outside autocast (pipeline.py:664
 [hi|lo|hi], weights [hi|hi|lo] along K, fp32 accumulation: all products but lo·lo, relative error ~2^-16 — the machinery of
 the Stage-II query path), activations and the residual stream stay fp32 between kernels, and the 257-token attention runs in
 fp32 on the CUDA cores (csrc/attention_small.cu).  The encoder is 2.5 TFLOP per clip against 16 400 for the denoise, so
-3x its GEMM work is invisible.  `precision="bf16"` keeps the round-1 path (bf16 operands, tcgen05 flash attention at
+3x its GEMM work is invisible.  `precision="bf16"` keeps the round-1 path (bf16 operands, wgmma flash attention at
 head_dim 64; last_hidden_state within 1e-2 of fp32).
 
 Image preprocessing (HF BitImageProcessor in the reference: bicubic resize to 256, centre crop 224, 1/255 rescale, ImageNet
@@ -93,7 +93,7 @@ class B200ImageEncoder:
     def to(self, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise AmbError("B200ImageEncoder runs on CUDA (sm_100a) only")
+            raise AmbError("B200ImageEncoder runs on CUDA (sm_90a) only")
         if device.index is None:
             device = torch.device("cuda", torch.cuda.current_device())
         self._device = device

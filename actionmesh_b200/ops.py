@@ -1,6 +1,6 @@
 """Torch-tensor front door to the C ABI (device pointers + the current CUDA stream; torch is only plumbing here).
 
-Every function launches hand-written sm_100a kernels from libactionmesh_b200.so; nothing here computes with torch ops.
+Every function launches hand-written sm_90a kernels from libactionmesh_b200.so; nothing here computes with torch ops.
 A global launch counter (`launch_count`) lets bench.py report how many of OUR kernels ran in the timed region.
 """
 from __future__ import annotations

@@ -239,7 +239,7 @@ def _vertex_normals(vertices: torch.Tensor, faces: torch.Tensor) -> torch.Tensor
 
 
 class ActionMeshB200Pipeline:
-    """Drop-in for `ActionMeshPipeline` on the B200 path: same constructor arguments, `.to(device)`, and `__call__`
+    """Drop-in for `ActionMeshPipeline` on the CUDA path: same constructor arguments, `.to(device)`, and `__call__`
     signature / return value (reference actionmesh/pipeline.py:47-53,205,602-685).
 
     Built from `actionmesh_b200.yaml` / `actionmesh_b200_fast.yaml` (the reference's YAML with the `_target_`s re-pointed):
@@ -298,7 +298,7 @@ class ActionMeshB200Pipeline:
     def to(self, device) -> "ActionMeshB200Pipeline":
         device = torch.device(device)
         if device.type != "cuda":
-            raise AmbError("ActionMeshB200Pipeline runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise AmbError("ActionMeshB200Pipeline runs on CUDA (sm_90a) only; there is no CPU fallback")
         self._target_device = device
         if not self._lazy_loading:
             self._load_image_encoder()

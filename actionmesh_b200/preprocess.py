@@ -140,7 +140,7 @@ class B200ImagePreprocessor:
         """frames (n, H, W, 3|4) uint8 (host or device) -> pixel_values (n, 3, crop_h, crop_w) fp32 on `device`."""
         dev = torch.device(device)
         if dev.type != "cuda":
-            raise AmbError("B200ImagePreprocessor only runs on a CUDA (sm_100) device; there is no CPU path")
+            raise AmbError("B200ImagePreprocessor only runs on a CUDA (sm_90) device; there is no CPU path")
         if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] not in (3, 4):
             raise AmbError(f"frames must be (n, H, W, 3|4) uint8, got {tuple(frames.shape)} {frames.dtype}")
         x = frames.contiguous()
@@ -194,7 +194,7 @@ class B200FramePreprocessor:
     def process_to_u8(self, frames: List) -> List[torch.Tensor]:
         """-> one (H', W', 3) uint8 CUDA tensor per frame (all the same size unless independent_cropping)."""
         if self.device.type != "cuda":
-            raise AmbError("B200FramePreprocessor only runs on a CUDA (sm_100) device; there is no CPU path")
+            raise AmbError("B200FramePreprocessor only runs on a CUDA (sm_90) device; there is no CPU path")
         arrs = [np.ascontiguousarray(f if getattr(f, "mode", "RGBA") == "RGBA" else f.convert("RGBA")) for f in frames]
         if len({a.shape for a in arrs}) != 1:
             raise AmbError("B200FramePreprocessor: all frames of a clip must have the same size")

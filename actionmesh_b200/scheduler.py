@@ -33,7 +33,7 @@ class B200SchedulerFlow:
     num_train_timesteps: int = 1000
     shift: float = 3.0
     is_additive: bool = False
-    split_cfg_batch: bool = False  # accepted for config compatibility; the B200 path never needs the split
+    split_cfg_batch: bool = False  # accepted for config compatibility; the CUDA path never needs the split
 
     # ---------------------------------------------------------------- schedule (host, float64 -> float32)
     def get_schedule(self) -> tuple[torch.Tensor, torch.Tensor]:

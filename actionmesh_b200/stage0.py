@@ -1,4 +1,4 @@
-"""Stage 0 on the B200 path — SURVEY 8(f) rank 2: TripoSG's DiT denoising loop, the step that produces the anchor latent
+"""Stage 0 on the CUDA path — SURVEY 8(f) rank 2: TripoSG's DiT denoising loop, the step that produces the anchor latent
 (reference actionmesh/pipeline.py:387-433 -> third_party/TripoSG).
 
 TripoSG's DiT (triposg/models/transformers/triposg_transformer.py:129-362,365-726) is the block family ActionMesh's

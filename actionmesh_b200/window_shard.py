@@ -47,10 +47,9 @@ def chunked_kv_views(kv_all: torch.Tensor, B: int, s_local: int, H: int, dh: int
 
 def configure_nccl_env() -> None:
     """Defaults for the per-layer K/V all-gather; call BEFORE `init_process_group` (NCCL caches its parameters at first use).
-    Measured with tools/shard_profile.py on 8x B200 (profiles/r01_shard_profile_8gpu.log): with NCCL's default choice the
-    235 MB gathers take 0.93 ms each next to the compute kernels and ~10 ms per step stay exposed; the Simple protocol on
-    32 channels brings them to 0.55 ms and the exposure to ~1 ms per step (step 91 -> 81 ms under the profiler).
-    Explicit user settings win (setdefault)."""
+    The Simple protocol on 32 channels was chosen on the project's first (Blackwell) target, where it cut the exposed gather
+    time per step about tenfold against NCCL's default choice (tools/shard_profile.py shows the timeline); it has not been
+    re-measured on H100s.  Explicit user settings win (setdefault)."""
     os.environ.setdefault("NCCL_PROTO", "Simple")
     os.environ.setdefault("NCCL_MIN_NCHANNELS", "32")
 
@@ -100,7 +99,7 @@ class PeerFrameShard(FrameShard):
 
     Why: next to SM-filling compute (persistent GEMMs, multi-wave attention) the cost of the all-gather is not its latency
     but its SMs — NCCL's 32-channel kernel runs concurrently with the other CFG branch's attention / MLP and inflates their
-    time (timeline: profiles/r01_shard_profile_8gpu.log).  DMA copies take no SM.
+    time (timeline: tools/shard_profile.py).  DMA copies take no SM.
 
     How: every rank's K/V projection writes into a symmetric-memory buffer (torch.distributed._symmetric_memory: one
     allocation per rank, mapped into every peer; `empty_kv_local` hands it to the denoiser's workspace).  `all_gather_kv`

@@ -1,13 +1,13 @@
-"""bench.py — denoiser steps/sec of the Stage-I temporal-3D-diffusion hot path (BASELINE.json metric) on N B200s.
+"""bench.py — denoiser steps/sec of the Stage-I temporal-3D-diffusion hot path (BASELINE.json metric) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--mode temporal|dp]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--mode temporal|dp] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 One "step" = one denoiser step of the default window (SURVEY 8(d), config c2): CFG batch of 2 branches x T=16 frames x
 N=2048 latent tokens (+1 time token) through the 21-block DiT (width 2048, 16 heads), CFG combine (7.5) + Euler update.
 5.469e14 algorithmic FLOP per step, of which the inflated self-attention QK^T+PV is 3.698e14 (BASELINE.md section 2).
 Weights are seeded-random (no checkpoints offline), inputs synthetic; the per-step working set (2.9 GB weights +
-GBs of activations) is far larger than the 126 MB L2, so no explicit L2 flush is needed between iterations.
+GBs of activations) is far larger than the 50 MB L2, so no explicit L2 flush is needed between iterations.
 
 Prints ONE JSON line (rank 0).
   N = 1: `value` = steps/s of the window on one GPU.
@@ -17,6 +17,9 @@ Prints ONE JSON line (rank 0).
          window per GPU, no collective, weak scaling — BASELINE config 4) the headline instead; either way the other figure
          is reported under `dp` / `temporal_shard`.
 `--impl reference` times the reference's own CPU path (the fp32 oracle port, all host threads) on a fixed bounded sample.
+`--dump-outputs DIR` writes, after the timed steps, the denoised latents of the timed window (what `denoise()` returns to
+its caller, (1, 16, 2048, 64) float32) as DIR/latents.npy.  Weights and inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -37,7 +40,7 @@ F_ATTN_LAUNCH = 4.0 * 2 * (16 * 2049) ** 2 * 2048   # one inflated self-attentio
 METRIC = "denoiser_steps_per_sec"
 UNIT = "steps/s"
 WORKLOAD = "davis_camel-shaped default window: CFG x2, T=16 frames, N=2048 tokens, 21-block DiT width 2048, guidance 7.5"
-ATTN_KERNEL = "flash_attn_pair_kernel (inflated self-attention, d_h 128, tcgen05 cta_group::2)"
+ATTN_KERNEL = "flash_attn_fwd_kernel<128> (inflated self-attention, d_h 128, wgmma)"
 T_WIN, N_TOK, C_LAT, S_CTX, D_CTX = 16, 2048, 64, 257, 1024
 CPU_SAMPLE_T = 8           # frames of the fixed CPU sample (identical in every run: BENCH, SCALE, --impl reference)
 
@@ -46,8 +49,8 @@ def _peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1380.2), d.get("hbm_gbs", 6570.3), "measured (MEASURED_PEAKS.json: sustained bf16 / hbm_gbs)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", NOMINAL_BF16_TF), d.get("hbm_gbs", NOMINAL_HBM_GBS), "measured (MEASURED_PEAKS.json: sustained bf16 / hbm_gbs)"
+    return NOMINAL_BF16_TF, NOMINAL_HBM_GBS, "H100 SXM data sheet (dense bf16, HBM3), not a measured figure"
 
 
 class ClockSampler:
@@ -154,7 +157,7 @@ def run_reference(args, rank: int):
 
 # ------------------------------------------------------------------------------------------------ reference recipe on the GPU
 def gpu_eager_baseline(dev, steps: int = 3) -> dict:
-    """The reference's own GPU recipe on the same B200: the oracle restatement of the reference modules (same op sequence:
+    """The reference's own GPU recipe on the same GPU: the oracle restatement of the reference modules (same op sequence:
     nn.Linear-equivalent matmuls, F.layer_norm, RMSNorm, RoPE, F.scaled_dot_product_attention, GELU) in PyTorch eager under
     torch.autocast(bf16) (pipeline.py:671), cuBLAS + torch's SDPA backend, plus the CFG combine / Euler update in torch."""
     import torch
@@ -200,7 +203,7 @@ def gpu_eager_baseline(dev, steps: int = 3) -> dict:
                     f"same window shape (torch {torch.__version__})"}
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------------ CUDA arm
 def run_b200(args):
     import torch
     import torch.distributed as dist
@@ -278,7 +281,8 @@ def run_b200(args):
         barrier()
         log = ops.event_log
         ops.event_log = None
-        return allmax(ev["t0"].elapsed_time(ev["t1"])), ops.launch_count - marks["launch0"], log, ev["t0"].elapsed_time(ev["t1"])
+        return (allmax(ev["t0"].elapsed_time(ev["t1"])), ops.launch_count - marks["launch0"], log, ev["t0"].elapsed_time(ev["t1"]),
+                lat)
 
     def timed_e2e(host_lat, host_ctx, use_shard):
         """The same metric through the public API with HOST buffers: inputs copied from pinned memory inside the timed region,
@@ -313,7 +317,7 @@ def run_b200(args):
     sampler = ClockSampler(local) if rank == 0 else None
     if temporal_main:
         hl, hc = host_inputs(0)                     # the SAME window on every rank
-        ms_total, launches, log, ms_local = timed_window(hl, hc, True, tags={"attn_self"})  # (few host cycles to spare per launch here)
+        ms_total, launches, log, ms_local, out = timed_window(hl, hc, True, tags={"attn_self"})  # (few host cycles to spare per launch here)
         value = K / (ms_total / 1e3)
         scaling = "strong"
         clocks = sampler.stop() if sampler else None
@@ -321,12 +325,19 @@ def run_b200(args):
         e2e_val = K / (e2e_ms / 1e3)
     else:
         hl, hc = host_inputs(rank)                  # one independent window per GPU
-        ms_total, launches, log, ms_local = timed_window(hl, hc, False, tags={"attn_self", "gemm", "layernorm"})
+        ms_total, launches, log, ms_local, out = timed_window(hl, hc, False, tags={"attn_self", "gemm", "layernorm"})
         value = world * K / (ms_total / 1e3)
         scaling = "weak"
         clocks = sampler.stop() if sampler else None
         e2e_ms, h2d, d2h = timed_e2e(hl, hc, False)
         e2e_val = world * K / (e2e_ms / 1e3)
+
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), out.detach().float().cpu().numpy())
+    del out
 
     # ---------------- N > 1: the other multi-GPU figure
     other = None
@@ -334,12 +345,12 @@ def run_b200(args):
         try:
             if temporal_main:
                 hl2, hc2 = host_inputs(rank)
-                ms2, _, _, _ = timed_window(hl2, hc2, False)
+                ms2 = timed_window(hl2, hc2, False)[0]
                 other = ("dp", {"value": world * K / (ms2 / 1e3), "unit": UNIT, "ms_per_step": ms2 / K, "scaling": "weak",
                                 "note": "whole-clip data parallel: one independent window per GPU, no data-path collective"})
             elif shard is not None:
                 hl2, hc2 = host_inputs(0)
-                ms2, _, _, _ = timed_window(hl2, hc2, True)
+                ms2 = timed_window(hl2, hc2, True)[0]
                 other = ("temporal_shard", {"value": K / (ms2 / 1e3), "unit": UNIT, "ms_per_step": ms2 / K, "scaling": "strong",
                                             "frames_per_rank": T // world,
                                             "note": "ONE window, frames sharded over the ranks, temporal-attention K/V all-gathered per layer"})
@@ -365,7 +376,7 @@ def run_b200(args):
             dist.destroy_process_group()
         return
     peak_tf, peak_hbm, peak_src = _peaks()
-    roof, roof_gemm, roof_ln = _rooflines(log or [], ms_local, peak_tf, peak_hbm, peak_src, world if temporal_main else 1)
+    roof, roof_gemm, roof_ln = _rooflines(log or [], ms_local, peak_tf, peak_hbm, peak_src)
     cpu = None
     if world == 1 and not args.no_cpu_baseline:
         cpu = cpu_baseline(repeats=3, warmup=1)
@@ -400,10 +411,11 @@ def run_b200(args):
         dist.destroy_process_group()
 
 
-NOMINAL_BF16_TF = 2250.0  # dense bf16 data-sheet peak of a B200 (the roofline denominator stays the MEASURED sustained figure)
+NOMINAL_BF16_TF = 989.0    # dense bf16 data-sheet peak of an H100 SXM at 700 W (the roofline denominator prefers a MEASURED figure)
+NOMINAL_HBM_GBS = 3350.0   # HBM3 data-sheet bandwidth of an H100 SXM
 
 
-def _rooflines(log, ms_local, peak_tf, peak_hbm, peak_src, attn_div):
+def _rooflines(log, ms_local, peak_tf, peak_hbm, peak_src):
     """Per-kernel-family roofline entries from the CUDA-event log of the timed region (events on the launching stream)."""
     by = {}
     for tag, e0, e1, meta in log:
@@ -415,26 +427,17 @@ def _rooflines(log, ms_local, peak_tf, peak_hbm, peak_src, attn_div):
         avg_ms = sum(a[0] for a in attn) / len(attn)
         fl = sum(4.0 * m[0] * m[1] * m[2] * m[3] * m[4] for _, m in attn) / len(attn)
         ach = fl / (avg_ms * 1e-3) / 1e12
-        tp = os.path.join(ROOT, "profiles", "attn_self_traffic.json")
-        traffic, tsrc = None, None
-        if os.path.exists(tp) and attn_div == 1:
-            tj = json.load(open(tp))
-            traffic, tsrc = tj.get("dram_bytes_per_launch"), "static: " + tj.get("source", "profiles/attn_self_traffic.json")
-        roof.update({"achieved": ach, "frac": ach / peak_tf, "traffic": traffic, "traffic_source": tsrc,
+        roof.update({"achieved": ach, "frac": ach / peak_tf,
                      "launches_timed": len(attn), "avg_launch_ms": avg_ms, "flops_per_launch": fl,
                      "share_of_step": sum(a[0] for a in attn) / ms_local,
                      "frac_of_nominal": ach / NOMINAL_BF16_TF})
-        if ach > peak_tf:
-            roof["note"] = ("above the pool's measured sustained cuBLAS bf16 figure: the step is power-capped and boxes of "
-                            "the pool differ by a few per cent in the clock they hold (see clocks); frac_of_nominal is "
-                            "against the 2250 TFLOP/s data-sheet peak")
     big = [(ms, m) for ms, m in by.get("gemm", []) if m[0] >= 4096]
     rg = None
     if big:
         fl = sum(2.0 * m[0] * m[1] * m[2] for _, m in big)
         tms = sum(ms for ms, _ in big)
         ach = fl / (tms * 1e-3) / 1e12
-        rg = {"bound": "tensor", "kernel": "gemm2_bf16_kernel / gemm_bf16_kernel (all nn.Linear of the block, fused epilogues)",
+        rg = {"bound": "tensor", "kernel": "gemm_bf16_kernel (all nn.Linear of the block, fused epilogues)",
               "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf, "traffic": None,
               "launches_timed": len(big), "share_of_step": tms / ms_local, "frac_of_nominal": ach / NOMINAL_BF16_TF}
     ln = [(ms, m) for ms, m in by.get("layernorm", []) if m[0] >= 4096]
@@ -530,6 +533,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-video", action="store_true")
     ap.add_argument("--no-eager", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the denoised latents of the timed window to DIR/latents.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args, int(os.environ.get("RANK", "0")))

@@ -1,5 +1,5 @@
 /*
- * actionmesh_b200 — C ABI of the B200-native (sm_100a) Stage-I denoising hot path of ActionMesh.
+ * actionmesh_b200 — C ABI of the H100-native (sm_90a) Stage-I denoising hot path of ActionMesh.
  *
  * The reference (facebookresearch/actionmesh) is pure Python on top of PyTorch library kernels; it has no FFI of its
  * own.  Each entry point below therefore cites the reference *call site* whose arithmetic it replaces (paths relative
@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define AMB_ABI_VERSION 13
+#define AMB_ABI_VERSION 14
 
 typedef void* amb_stream_t; /* cudaStream_t */
 
@@ -129,12 +129,12 @@ int amb_split3_bf16(const float* src, int64_t ld_src, int64_t rows, int cols, in
 int amb_softmax_split3(const float* scores, int64_t ld_s, int rows, int n, int n_pad, float scale, void* dst_bf16,
                        int64_t ld_dst, amb_stream_t stream);
 
-/* ---- tcgen05 GEMM with fused epilogues: C = epi(A · Wᵀ) ----------------------------------------------------------------
+/* ---- wgmma GEMM with fused epilogues: C = epi(A · Wᵀ) ----------------------------------------------------------------
  * Replaces every nn.Linear on the path (cuBLAS in the reference): proj_in/proj_out/time_proj
  * (temporal_denoiser.py:206,213-214,242), linear_skip on cat[skip,h] without materialising the concat (block.py:131-133,
  * a2/k_split), to_q/to_k/to_v with the head split, RMS qk-norm and RoPE of attention_processor.py:92-130 fused in the
  * epilogue, to_out + residual (attention_processor.py:147, block.py:137,146), FeedForward GELU(erf) MLP (block.py:152).
- * A:(m,k) bf16 row-major, W:(n,k) bf16 row-major (nn.Linear layout), fp32 accumulation in TMEM.
+ * A:(m,k) bf16 row-major, W:(n,k) bf16 row-major (nn.Linear layout), fp32 accumulation in registers.
  * k % 64 == 0, n % 64 == 0.
  */
 typedef struct amb_gemm_args {
@@ -177,7 +177,7 @@ typedef struct amb_gemm_args {
 
 int amb_gemm_bf16(const amb_gemm_args* args, amb_stream_t stream);
 
-/* ---- tcgen05 flash attention forward ------------------------------------------------------------------------------
+/* ---- wgmma flash attention forward -------------------------------------------------------------------------------
  * Replaces F.scaled_dot_product_attention at actionmesh/model/utils/attention_processor.py:133-139 (non-causal, no
  * mask, dropout 0) for the inflated self-attention (S = T*(N+1)) and the per-frame cross-attention (S_k = 257), and
  * DinoV2's attention (head_dim 64).  Strided 4-D views so q/k/v are read straight out of the fused QKV GEMM output and
@@ -209,10 +209,6 @@ int amb_flash_attn_fwd(const amb_attn_args* args, amb_stream_t stream);
  * seq <= 320.  No mask, non-causal; softmax(scale * q k^T) v with fp32 arithmetic throughout (CUDA cores). */
 int amb_attn_small_f32(const float* q, const float* k, const float* v, int64_t ld, int frames, int seq, int heads, float scale,
                        float* out, int64_t ldo, amb_stream_t stream);
-
-/* Debug only: device buffer (5 roles x 16 iterations x 8 events of int64 clock64 stamps) receiving the role timeline of
- * CTA (0,0,0) of the head_dim-128 attention kernel; NULL switches tracing off (the default). */
-int amb_debug_set_attn_trace(void* device_buffer);
 
 #ifdef __cplusplus
 }

@@ -110,7 +110,7 @@ def main():
                os.path.join(GOLD, "denoiser_tiny_autocast.pt"))
 
     # ---- the same pair of trajectories (fp32 and the reference's bf16 autocast recipe) for 8 (weight seed, input seed)
-    # draws: tests/test_chamfer_gpu.py compares the B200 path's Chamfer with the reference-autocast Chamfer in the MEAN
+    # draws: tests/test_chamfer_gpu.py compares the CUDA path's Chamfer with the reference-autocast Chamfer in the MEAN
     multi = {"config": TINY, "pairs": []}
     for ws, isd in MULTI_SEEDS:
         mm = _model(ns, TINY, ws)
@@ -180,8 +180,82 @@ def main():
                 "timesteps": sched.timesteps.clone(), "sigmas": sched.sigmas.clone(), "denoise4_cfg2_out": lat,
                 "state_dict_keys": sorted(tri.state_dict().keys())}, os.path.join(GOLD, "triposg_tiny.pt"))
 
+    live_reference(ns, tns)
+
     for f in sorted(os.listdir(GOLD)):
         print(f, os.path.getsize(os.path.join(GOLD, f)))
+
+
+def live_reference(ns=None, tns=None):
+    """tests/golden/live_reference.pt: what the tests that used to import the reference checkout compared against — the
+    reference denoiser's forward and `chunk_from` partitions, its ImagePreprocessor output, the key tree and values of its
+    YAML configs, and the TripoSG RectifiedFlowScheduler tables."""
+    import importlib.util
+
+    from actionmesh_b200.config import load_config
+
+    ns = ns or reference_loader.load()
+    tns = tns or reference_loader.load_triposg()
+    torch.set_grad_enabled(False)
+    live = {}
+
+    # ---- denoiser forward at a small width + chunk_from (tests/test_oracle_golden.py)
+    d = dict(num_layers=3, num_attention_heads=2, width=256, cross_attention_dim=64, in_channels=64, mlp_ratio=2.0)
+    m = ns.ActionMeshDenoiser(inflated_layers=(0, 1, 2), **d).eval()
+    m.load_state_dict(synth.make_state_dict(m, 9), strict=True)
+    lat, ctx, fs, mask = synth.make_inputs(2, 4, 7, 64, 5, 64, seed=11, observed=(1,))
+    out, _ = m.forward(hidden_states=lat, context=ctx, framestep=fs, diffusion_time=torch.tensor([300.0, 300.0]), mask=mask)
+    chunks = {}
+    for total in (16, 17, 31, 32, 47, 64):
+        for start in (0, 3, total // 2, total - 1):
+            chunks[(start, total)] = ns.chunk_from(start, total, 16, 15)
+    live["denoiser"] = {"config": d, "seed": 9, "input_seed": 11, "forward_out": out, "state_dict_keys": sorted(m.state_dict()),
+                        "chunk_from": chunks}
+
+    # ---- ImagePreprocessor.process_images on the frames of tests/test_frame_preprocess.py
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from PIL import Image
+    from test_frame_preprocess import _frames
+
+    spec = importlib.util.spec_from_file_location(
+        "ref_image_processor", os.path.join(reference_loader.REFERENCE_ROOT, "actionmesh", "preprocessing", "image_processor.py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    import numpy as np
+
+    live["frame_preprocess"] = {
+        ind: [np.asarray(a).copy() for a in mod.ImagePreprocessor(independent_cropping=ind, padding_ratio=0.1).process_images(
+            [Image.fromarray(f, "RGBA") for f in _frames()])]
+        for ind in (False, True)}
+
+    # ---- YAML configs (tests/test_config_cpu.py): every key path and the values the tests compare
+    cfg_dir = os.path.join(reference_loader.REFERENCE_ROOT, "actionmesh", "configs")
+    ref = load_config("actionmesh.yaml", cfg_dir)
+    fast = load_config("actionmesh_fast.yaml", cfg_dir)
+
+    def keys(node, prefix=""):
+        out = set()
+        for k, v in node.items():
+            out.add(prefix + k)
+            if isinstance(v, dict):
+                out |= keys(v, prefix + k + ".")
+        return out
+
+    top = ("stage_0_steps", "face_decimation", "floaters_threshold", "stage_1_steps", "anchor_idx", "sliding_window_denoiser",
+           "subsampling_level", "sliding_window_autoencoder")
+    live["config"] = {"keys": sorted(keys(ref)), "top": {k: ref[k] for k in top},
+                      "blocks": {blk: {k: v for k, v in ref.model[blk].items() if k != "_target_"} for blk in ("scheduler", "cf_guidance")},
+                      "fast_stage_1_steps": fast.stage_1_steps,
+                      "fast_scheduler_steps": fast.model.scheduler.num_inference_steps}
+
+    # ---- TripoSG RectifiedFlowScheduler tables (tests/test_stage0_cpu.py)
+    sched = {}
+    for n, shift in ((50, 1.0), (100, 3.0), (7, 2.5)):
+        r = tns.RectifiedFlowScheduler(num_train_timesteps=1000, shift=shift)
+        r.set_timesteps(n)
+        sched[(n, shift)] = (r.timesteps.clone(), r.sigmas.clone())
+    live["rectified_flow"] = sched
+    torch.save(live, os.path.join(GOLD, "live_reference.pt"))
 
 
 if __name__ == "__main__":

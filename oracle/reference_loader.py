@@ -1,7 +1,6 @@
-"""TEST INFRASTRUCTURE ONLY.  Import the reference's OWN hot-path modules unchanged from /root/reference.
-
-Only usable in the build container (the GPU box has no /root/reference).  Used by gen_golden.py and by the CPU tests
-that pin oracle/denoiser_oracle.py against the reference's code.
+"""TEST INFRASTRUCTURE ONLY.  Import the reference's OWN hot-path modules unchanged from a checkout of
+facebookresearch/actionmesh (path in $ACTIONMESH_REFERENCE).  Used by gen_golden.py, which stores what those modules return
+under tests/golden/; the tests themselves never need the checkout.
 """
 from __future__ import annotations
 

@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -21,7 +21,7 @@ def golden_dir():
 
 @pytest.fixture(scope="session")
 def amb_lib():
-    """The sm_100a C-ABI library; built on demand (nvcc cross-compiles without a GPU)."""
+    """The sm_90a C-ABI library; built on demand (nvcc cross-compiles without a GPU)."""
     import __graft_entry__ as ge
 
     if not os.path.exists(ge.LIB_PATH):

@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 denoiser / scheduler against the fp32 oracle and the committed golden fixtures
+"""End-to-end parity of the CUDA denoiser / scheduler against the fp32 oracle and the committed golden fixtures
 (reference outputs) on the GPU (-m gpu).
 
 Tolerance (stated once): the CUDA path keeps the residual stream, GEMM operands and attention probabilities in bf16 with

@@ -1,18 +1,15 @@
 """ImagePreprocessor (composite on white, crop to the foreground box, pad to a square) — SURVEY 8(f) rank 3, second half.
 
-CPU: the numpy restatement (oracle/preprocess_oracle.py) against the reference's OWN `ImagePreprocessor.process_images`
-(actionmesh/preprocessing/image_processor.py, loaded by file path; needs only numpy/torch/PIL) when the checkout is present.
+CPU: the numpy restatement (oracle/preprocess_oracle.py) against the output of the reference's OWN
+`ImagePreprocessor.process_images` (actionmesh/preprocessing/image_processor.py) on the frames below, stored by
+oracle/gen_golden.py in tests/golden/live_reference.pt.
 GPU (-m gpu): B200FramePreprocessor's uint8 output `array_equal` to the restatement, shared and independent cropping,
 non-square frames, the invalid-alpha error."""
-import importlib.util
-import os
-
 import numpy as np
 import pytest
 
+from conftest import load_golden
 from oracle import preprocess_oracle
-
-REF = "/root/reference/actionmesh/preprocessing/image_processor.py"
 
 
 def _frames(n=5, H=96, W=128, seed=3):
@@ -29,17 +26,10 @@ def _frames(n=5, H=96, W=128, seed=3):
     return out
 
 
-@pytest.mark.skipif(not os.path.exists(REF), reason="reference checkout not present")
 @pytest.mark.parametrize("independent", [False, True])
 def test_restatement_matches_the_reference_module(independent):
-    from PIL import Image
-
-    spec = importlib.util.spec_from_file_location("ref_image_processor", REF)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
+    ref = load_golden("live_reference.pt")["frame_preprocess"][independent]
     frames = _frames()
-    ref = mod.ImagePreprocessor(independent_cropping=independent, padding_ratio=0.1).process_images(
-        [Image.fromarray(f, "RGBA") for f in frames])
     ours = preprocess_oracle.frame_preprocess(frames, independent, 0.1)
     assert len(ref) == len(ours)
     for a, b in zip(ref, ours):

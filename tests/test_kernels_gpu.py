@@ -1,4 +1,4 @@
-"""Kernel parity on the B200 (-m gpu): every C-ABI compute entry point against a torch fp32 reference of the same op
+"""Kernel parity on the GPU (-m gpu): every C-ABI compute entry point against a torch fp32 reference of the same op
 on seeded inputs.  Tolerances: outputs are bf16, so relative Frobenius error <= 4e-3 (bf16 has 8 mantissa bits,
 2^-9 = 1.95e-3 per rounding; two roundings on the fused paths) unless the output is fp32 (1e-5)."""
 import math
@@ -99,12 +99,10 @@ def test_gemm_is_linear_in_a(probe):
     ("d64_s257", (3, 4, 257, 257, 64), {}),
     ("d64_fused", (2, 16, 257, 257, 64), dict(fused=True)),
     ("window_t2", (2, 16, 2 * 2049, 2 * 2049, 128), dict(fused=True)),
-    # >= 48 key tiles: the CTA-pair kernel.  Logits with std 8 push most rows out of the fixed-reference safe range, so the
-    # units are marked dirty by the fast pass and recomputed by the exact pass launched behind it (ragged q and key tails)
+    # 50 key tiles: long key loops.  Logits with std 8 move every row's running maximum many times (ragged q and key tails)
     ("pair_dirty_units_fixup", (1, 2, 300, 128 * 50 + 17, 128), dict(mode="sharp8")),
     ("pair_clean_ragged", (2, 2, 300, 128 * 50 + 17, 128), {}),
-    # one key far above the row reference, in a key slot whose exp2 is the FMA-pipe polynomial: must be caught (argument clamp
-    # at 127 -> 2^127 -> row-sum range check) and the unit redone exactly; the output is then v of that key
+    # one key far above every other: the running maximum jumps on that key's tile and the output is v of that key
     ("pair_single_spike_key", (1, 2, 300, 128 * 50, 128), dict(mode="spike")),
 ])
 def test_flash_attention(probe, name, args, kw):
@@ -123,7 +121,7 @@ def test_flash_attention_late_rescale(probe):
 
 
 def test_flash_attention_late_rescale_pair_kernel(probe):
-    """The same construction over 50 key tiles: the CTA-pair kernel, every unit dirty, exact pass with in-loop rescales."""
+    """The same construction over 50 key tiles: a rescale of the running output on every tile of a long key loop."""
     _late_rescale_case(probe, 128 * 50 + 17)
 
 

@@ -1,4 +1,4 @@
-"""Stage 0 on the B200 (-m gpu): B200TripoSGDiT / TripoSGStage0 against the fixture written by the reference's own
+"""Stage 0 on the GPU (-m gpu): B200TripoSGDiT / TripoSGStage0 against the fixture written by the reference's own
 TripoSGDiTModel + RectifiedFlowScheduler in fp32 (tests/golden/triposg_tiny.pt).  Tolerances as for the Stage-I denoiser
 (bf16 GEMM / attention operands, fp32 accumulation and residual stream): one forward 2e-2, 4-step CFG trajectory 3e-2."""
 import pytest

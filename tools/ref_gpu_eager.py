@@ -1,4 +1,4 @@
-"""Reference-equivalent PyTorch-eager timing on the B200 (context for BASELINE.md; not part of the product).
+"""Reference-equivalent PyTorch-eager timing on the GPU (context for BASELINE.md; not part of the product).
 
 Runs the oracle restatement of the reference's denoiser forward (same op sequence as the reference's modules:
 nn.Linear-equivalent matmuls, F.layer_norm, RMSNorm, RoPE, F.scaled_dot_product_attention, GELU) on CUDA under

@@ -89,7 +89,7 @@ def main():
         e1.record()
         sync()
         lat, _ = bank.get_ordered()
-        out = {"config": "c3: --fast scheduler (15 steps), 32-frame synthetic video, bf16 operands, 1xB200", "frames": n_frames,
+        out = {"config": "c3: --fast scheduler (15 steps), 32-frame synthetic video, bf16 operands, 1xH100", "frames": n_frames,
                "windows": n_windows, "steps_per_window": steps, "denoiser_steps": n_windows * steps,
                "stage1_seconds": e0.elapsed_time(e1) / 1e3, "steps_per_sec": n_windows * steps / (e0.elapsed_time(e1) / 1e3),
                "finite": bool(torch.isfinite(lat).all()), "latents_shape": list(lat.shape),
@@ -110,7 +110,7 @@ def main():
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         sec = float(t.item()) / 1e3
-        out = {"config": f"c4: ActionBench-style batch, whole-clip data parallel across {world}xB200 (no data-path collective)",
+        out = {"config": f"c4: ActionBench-style batch, whole-clip data parallel across {world}xH100 (no data-path collective)",
                "clips_run": per_rank * world, "clips_per_gpu": per_rank, "steps_per_clip": steps, "seconds": sec,
                "clips_per_sec": per_rank * world / sec, "denoiser_steps_per_sec": per_rank * world * steps / sec,
                "projected_seconds_128_clips": 128 / (per_rank * world / sec)}
@@ -130,7 +130,7 @@ def main():
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         sec = float(t.item()) / 1e3
         lat, _ = bank.get_ordered()
-        out = {"config": f"c5: single 256-frame synthetic video, 17 serial AR windows, each window's frames sharded across {world}xB200 "
+        out = {"config": f"c5: single 256-frame synthetic video, 17 serial AR windows, each window's frames sharded across {world}xH100 "
                          f"({'copy-engine peer copies' if args.exchange == 'peer' else 'NCCL all-gather'} of the temporal-attention K/V)",
                "frames": n_frames, "windows": len(windows), "steps_per_window": steps, "denoiser_steps": len(windows) * steps,
                "seconds": sec, "steps_per_sec": len(windows) * steps / sec, "finite": bool(torch.isfinite(lat).all()),
