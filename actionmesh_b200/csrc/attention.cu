@@ -4,12 +4,16 @@
 //
 // One CTA owns 128 query rows of one (batch, head); three warpgroups:
 //   warpgroup 0     TMA producer: the Q tile once, then a STAGES-deep ring of 128-key K and V tiles (strided 4-D / 5-D tensor
-//                   maps, so q/k/v are read in place from the fused QKV GEMM output; K and V on separate barriers so that
-//                   Q·Kᵀ starts before V has landed)
+//                   maps, so q/k/v are read in place from the fused QKV GEMM output).  K and V have their own full and empty
+//                   barriers: Q·Kᵀ starts before V has landed, and a K slot is refilled as soon as its S = Q·Kᵀ is done.
+//                   It also watches the consumers for a stall (bounded wait and trap), since they hold 240 registers and
+//                   ptxas allocates fewer to a warp that can trap.
 //   warpgroups 1-2  consumers, 64 query rows each:  S = Q·Kᵀ (wgmma, both operands in shared memory) -> online softmax in
 //                   registers (exp2 with the scale folded in; a row lives in one quad, so its max / sum are two shuffles) ->
-//                   O += P·V (wgmma with P as the register A operand, V MN-major from shared memory).  The two consumer
-//                   warpgroups interleave: one computes exponentials while the other's MMAs run.
+//                   O += P·V (wgmma with P as the register A operand, V MN-major from shared memory).
+// The consumers are software-pipelined: S_{j+1} = Q·K_{j+1}ᵀ and O += P_j·V_j are issued together, and the softmax of S_{j+1}
+// runs while P_j·V_j is still on the tensor cores.  The two consumer warpgroups take turns issuing their MMAs (named
+// barriers 1 and 2), so one warpgroup's softmax also overlaps the other's MMAs.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "attention.cuh"
@@ -30,14 +34,83 @@ struct AttnSmem {
   static constexpr int K_OFF = Q_BYTES;
   static constexpr int V_OFF = K_OFF + ATT_STAGES * KV_BYTES;
   static constexpr int BAR_OFF = V_OFF + ATT_STAGES * KV_BYTES;
-  static constexpr int NUM_BARS = 1 + 3 * ATT_STAGES;            // q_full, k_full[], v_full[], kv_empty[]
+  static constexpr int NUM_BARS = 1 + 4 * ATT_STAGES;            // q_full, k_full[], v_full[], k_empty[], v_empty[]
   static constexpr int TOTAL = BAR_OFF + NUM_BARS * 8 + 1024;
 };
 
+// S = Q·K_sᵀ for one warpgroup (64 x 128): 16 columns of d per k16 step, +32 B inside a 128-B row, next box after 4 steps.
+// The first step overwrites the accumulator (scale-d 0).
 template <int D>
-__device__ __forceinline__ void pv_k16(float* o, const uint32_t* a, uint64_t vdesc) {
-  if constexpr (D == 128) wgmma_rs_n128_tb(o, a, vdesc, 1u);
-  else wgmma_rs_n64_tb(o, a, vdesc, 1u);
+__device__ __forceinline__ void qk_issue(float* sc, uint32_t sq_addr, uint32_t sk_addr) {
+#pragma unroll
+  for (int k = 0; k < D / 16; ++k) {
+    const uint32_t off = (k >> 2) * AttnSmem<D>::BOX_BYTES + (k & 3) * 32;
+    wgmma_ss_n128(sc, make_desc_kmajor_sw128(sq_addr + off), make_desc_kmajor_sw128(sk_addr + off), k > 0 ? 1u : 0u);
+  }
+  wgmma_commit();
+}
+
+// O += P·V_s: 16 keys per step = 2048 B of the MN-major V tile; the second 64-column box of d is BOX_BYTES further.
+template <int D>
+__device__ __forceinline__ void pv_issue(float* o, const uint32_t* pk, uint32_t sv_addr) {
+#pragma unroll
+  for (int kk = 0; kk < ATT_BK / 16; ++kk) {
+    const uint64_t vdesc = make_desc_mnmajor_sw128(sv_addr + kk * 2048, AttnSmem<D>::BOX_BYTES);
+    if constexpr (D == 128) wgmma_rs_n128_tb(o, pk + 4 * kk, vdesc, 1u);
+    else wgmma_rs_n64_tb(o, pk + 4 * kk, vdesc, 1u);
+  }
+  wgmma_commit();
+}
+
+// Online-softmax update with one S tile (sc[4i + {0,1}] = row a, keys 8i + 2q + {0,1}; sc[4i + {2,3}] = row b, same keys):
+// keys >= valid are masked, the running maxima m rise, sc becomes exp2((S - m)·c), its row sums are added to l, and al gets
+// the factors exp2((m_old - m)·c) that rescale the older terms (0 on the first tile).
+__device__ __forceinline__ void softmax_tile(float* sc, int valid, int q, float c, float& m_a, float& m_b, float& l_a,
+                                             float& l_b, float& al_a, float& al_b) {
+  if (valid < ATT_BK) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int key = 8 * i + 2 * q;
+      if (key >= valid) sc[4 * i] = sc[4 * i + 2] = -INFINITY;
+      if (key + 1 >= valid) sc[4 * i + 1] = sc[4 * i + 3] = -INFINITY;
+    }
+  }
+  float mx_a = m_a, mx_b = m_b;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    mx_a = fmaxf(mx_a, fmaxf(sc[4 * i], sc[4 * i + 1]));
+    mx_b = fmaxf(mx_b, fmaxf(sc[4 * i + 2], sc[4 * i + 3]));
+  }
+  mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1));
+  mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1));
+  mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
+  mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
+  al_a = ex2_approx((m_a - mx_a) * c);
+  al_b = ex2_approx((m_b - mx_b) * c);
+  m_a = mx_a;
+  m_b = mx_b;
+  const float mb_a = m_a * c, mb_b = m_b * c;
+  float ts_a = 0.f, ts_b = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    sc[4 * i] = ex2_approx(fmaf(sc[4 * i], c, -mb_a));
+    sc[4 * i + 1] = ex2_approx(fmaf(sc[4 * i + 1], c, -mb_a));
+    sc[4 * i + 2] = ex2_approx(fmaf(sc[4 * i + 2], c, -mb_b));
+    sc[4 * i + 3] = ex2_approx(fmaf(sc[4 * i + 3], c, -mb_b));
+    ts_a += sc[4 * i] + sc[4 * i + 1];
+    ts_b += sc[4 * i + 2] + sc[4 * i + 3];
+  }
+  l_a = l_a * al_a + ts_a;
+  l_b = l_b * al_b + ts_b;
+}
+
+// A fragment of P·V from the exponentials: (row a, keys 2q, 2q+1) / (row b, ...) of 8-key group i.
+__device__ __forceinline__ void pack_p(uint32_t* pk, const float* sc) {
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    pk[2 * i] = pack_bf16(sc[4 * i], sc[4 * i + 1]);
+    pk[2 * i + 1] = pack_bf16(sc[4 * i + 2], sc[4 * i + 3]);
+  }
 }
 
 template <int D>
@@ -51,7 +124,8 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* k_full = q_full + 1;
   uint64_t* v_full = k_full + ATT_STAGES;
-  uint64_t* kv_empty = v_full + ATT_STAGES;
+  uint64_t* k_empty = v_full + ATT_STAGES;
+  uint64_t* v_empty = k_empty + ATT_STAGES;
 
   const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);  // warp-uniform role
   const int warp = threadIdx.x >> 5;
@@ -70,7 +144,8 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     for (int s = 0; s < ATT_STAGES; ++s) {
       mbar_init(&k_full[s], 1);
       mbar_init(&v_full[s], 1);
-      mbar_init(&kv_empty[s], 8);  // one arrival per consumer warp
+      mbar_init(&k_empty[s], 8);  // one arrival per consumer warp
+      mbar_init(&v_empty[s], 8);
     }
     fence_mbar_init();
   }
@@ -88,21 +163,32 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
       __syncwarp();
       int s = 0;
       uint32_t phase = 0;
-      for (int j = 0; j < n_kv; ++j) {
+      for (int j = 0; j < n_kv; ++j) {  // K/V maps are 5-D: (d, key, head, batch, chunk)
         const int chunk = j / tiles_per_chunk;
         const int key0 = (j - chunk * tiles_per_chunk) * ATT_BK;
-        mbar_wait(&kv_empty[s], phase ^ 1);
-        if (elect_one()) {  // K/V maps are 5-D: (d, key, head, batch, chunk)
+        mbar_wait(&k_empty[s], phase ^ 1);  // K_j's slot frees before V_j's: load it first
+        if (elect_one()) {
           uint8_t* sk = smem + L::K_OFF + s * L::KV_BYTES;
-          uint8_t* sv = smem + L::V_OFF + s * L::KV_BYTES;
           mbar_expect_tx(&k_full[s], L::KV_BYTES);
           for (int c = 0; c < DH; ++c)
             tma_load_5d(sk + c * L::BOX_BYTES, &tmK, &k_full[s], c * 64, key0, head, batch, chunk, kEvictLast);
+        }
+        __syncwarp();
+        mbar_wait(&v_empty[s], phase ^ 1);
+        if (elect_one()) {
+          uint8_t* sv = smem + L::V_OFF + s * L::KV_BYTES;
           mbar_expect_tx(&v_full[s], L::KV_BYTES);
           for (int c = 0; c < DH; ++c)
             tma_load_5d(sv + c * L::BOX_BYTES, &tmV, &v_full[s], c * 64, key0, head, batch, chunk, kEvictLast);
         }
         __syncwarp();
+        if (++s == ATT_STAGES) { s = 0; phase ^= 1; }
+      }
+      // Watchdog: the consumers wait without a timeout (see mbar_wait_watched), so this warp waits, bounded, until they
+      // have released the last STAGES tiles.  A stalled consumer makes that wait trap and the launch fail.
+      for (int j = 0; j < ATT_STAGES; ++j) {
+        mbar_wait(&k_empty[s], phase ^ 1);
+        mbar_wait(&v_empty[s], phase ^ 1);
         if (++s == ATT_STAGES) { s = 0; phase ^= 1; }
       }
     }
@@ -116,70 +202,63 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     const uint32_t sv_addr = smem_u32(smem + L::V_OFF);
     const float c = p.scale_log2;
     const int last_valid = p.sk_chunk - (tiles_per_chunk - 1) * ATT_BK;  // valid keys in the last tile of each chunk
+    // Issue turns: warpgroup w waits on named barrier w before issuing and then lets the other one go.  Warpgroup 1 takes the
+    // first turn without waiting and warpgroup 2 gives no go-ahead after its last turn, so every arrival is matched by a wait.
+    const uint32_t my_turn = wg, other_turn = 3 - wg;
 
     float o[D / 2];
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
     float m_a = -INFINITY, m_b = -INFINITY;  // running maxima (raw score units) of my two rows
     float l_a = 0.f, l_b = 0.f;              // partial row sums over my columns
+    float al_a, al_b;
+    float sc[64];
+    uint32_t pk[32];
 
-    mbar_wait(q_full, 0);
-    int s = 0, jj = 0;
+    // ---- prologue: S_0 and its softmax (O is still zero: nothing to rescale)
+    mbar_wait_watched(q_full, 0);
+    mbar_wait_watched(&k_full[0], 0);
+    if (wg == 2) named_bar_sync(my_turn, 256);
+    wgmma_fence();
+    qk_issue<D>(sc, sq_addr, sk_addr);
+    named_bar_arrive(other_turn, 256);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 64; ++i) reg_fence(sc[i]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&k_empty[0]);  // this warp is done with K_0
+    int jn = tiles_per_chunk == 1 ? 0 : 1;    // tile index inside its chunk of the NEXT tile
+    softmax_tile(sc, tiles_per_chunk == 1 ? last_valid : ATT_BK, q, c, m_a, m_b, l_a, l_b, al_a, al_b);
+    pack_p(pk, sc);
+
+    int s = 0;
     uint32_t phase = 0;
-    for (int j = 0; j < n_kv; ++j) {
-      // ---- S = Q Kᵀ (64 x 128 per warpgroup)
-      float sc[64];
-#pragma unroll
-      for (int i = 0; i < 64; ++i) sc[i] = 0.f;
-      mbar_wait(&k_full[s], phase);
+    for (int j = 0; j + 1 < n_kv; ++j) {
+      int sn = s + 1;
+      uint32_t phn = phase;
+      if (sn == ATT_STAGES) { sn = 0; phn ^= 1; }
+      // ---- issue S_{j+1} = Q·K_{j+1}ᵀ, then O += P_j·V_j
+      mbar_wait_watched(&k_full[sn], phn);
+      mbar_wait_watched(&v_full[s], phase);
+      named_bar_sync(my_turn, 256);
       wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < D / 16; ++k) {  // 16 columns of d per step: +32 B inside a 128-B row, next box after 4 steps
-        const uint32_t off = (k >> 2) * L::BOX_BYTES + (k & 3) * 32;
-        wgmma_ss_n128(sc, make_desc_kmajor_sw128(sq_addr + off), make_desc_kmajor_sw128(sk_addr + s * L::KV_BYTES + off), 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
+      qk_issue<D>(sc, sq_addr, sk_addr + sn * L::KV_BYTES);
+      pv_issue<D>(o, pk, sv_addr + s * L::KV_BYTES);
+      named_bar_arrive(other_turn, 256);
+      // ---- softmax of S_{j+1} while P_j·V_j runs
+      wgmma_wait<1>();
 #pragma unroll
       for (int i = 0; i < 64; ++i) reg_fence(sc[i]);
-
-      // ---- online softmax: sc[4i + {0,1}] = row a, keys 8i + 2q + {0,1}; sc[4i + {2,3}] = row b, same keys
-      if (jj == tiles_per_chunk - 1 && last_valid < ATT_BK) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&k_empty[sn]);
+      softmax_tile(sc, jn == tiles_per_chunk - 1 ? last_valid : ATT_BK, q, c, m_a, m_b, l_a, l_b, al_a, al_b);
+      if (++jn == tiles_per_chunk) jn = 0;
+      // ---- P_j·V_j done: release V_j, rescale O for tile j+1 and pack P_{j+1}
+      wgmma_wait<0>();
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int key = 8 * i + 2 * q;
-          if (key >= last_valid) sc[4 * i] = sc[4 * i + 2] = -INFINITY;
-          if (key + 1 >= last_valid) sc[4 * i + 1] = sc[4 * i + 3] = -INFINITY;
-        }
-      }
-      if (++jj == tiles_per_chunk) jj = 0;
-      float mx_a = m_a, mx_b = m_b;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        mx_a = fmaxf(mx_a, fmaxf(sc[4 * i], sc[4 * i + 1]));
-        mx_b = fmaxf(mx_b, fmaxf(sc[4 * i + 2], sc[4 * i + 3]));
-      }
-      mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1));
-      mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1));
-      mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
-      mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
-      const float al_a = ex2_approx((m_a - mx_a) * c), al_b = ex2_approx((m_b - mx_b) * c);  // 0 on the first tile
-      m_a = mx_a;
-      m_b = mx_b;
-      const float mb_a = m_a * c, mb_b = m_b * c;
-      uint32_t pk[32];
-      float ts_a = 0.f, ts_b = 0.f;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const float ea0 = ex2_approx(fmaf(sc[4 * i], c, -mb_a)), ea1 = ex2_approx(fmaf(sc[4 * i + 1], c, -mb_a));
-        const float eb0 = ex2_approx(fmaf(sc[4 * i + 2], c, -mb_b)), eb1 = ex2_approx(fmaf(sc[4 * i + 3], c, -mb_b));
-        ts_a += ea0 + ea1;
-        ts_b += eb0 + eb1;
-        pk[2 * i] = pack_bf16(ea0, ea1);      // A fragment of P·V: (row a, keys 2q, 2q+1) / (row b, ...) of 8-key group i
-        pk[2 * i + 1] = pack_bf16(eb0, eb1);
-      }
-      l_a = l_a * al_a + ts_a;
-      l_b = l_b * al_b + ts_b;
+      for (int i = 0; i < D / 2; ++i) reg_fence(o[i]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&v_empty[s]);
 #pragma unroll
       for (int i = 0; i < D / 8; ++i) {
         o[4 * i] *= al_a;
@@ -187,22 +266,22 @@ flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         o[4 * i + 2] *= al_b;
         o[4 * i + 3] *= al_b;
       }
-
-      // ---- O += P V: 16 keys per step = 2048 B of the MN-major V tile; the second 64-column box of d is BOX_BYTES further
-      mbar_wait(&v_full[s], phase);
-      wgmma_fence();
-      const uint32_t vbase = sv_addr + s * L::KV_BYTES;
-#pragma unroll
-      for (int kk = 0; kk < ATT_BK / 16; ++kk)
-        pv_k16<D>(o, pk + 4 * kk, make_desc_mnmajor_sw128(vbase + kk * 2048, L::BOX_BYTES));
-      wgmma_commit();
-      wgmma_wait<0>();
-#pragma unroll
-      for (int i = 0; i < D / 2; ++i) reg_fence(o[i]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&kv_empty[s]);  // this warp is done with K_j and V_j
-      if (++s == ATT_STAGES) { s = 0; phase ^= 1; }
+      pack_p(pk, sc);
+      s = sn;
+      phase = phn;
     }
+
+    // ---- last tile: O += P·V
+    mbar_wait_watched(&v_full[s], phase);
+    named_bar_sync(my_turn, 256);
+    wgmma_fence();
+    pv_issue<D>(o, pk, sv_addr + s * L::KV_BYTES);
+    if (wg == 1) named_bar_arrive(other_turn, 256);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) reg_fence(o[i]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&v_empty[s]);
 
     // ---- epilogue: O / rowsum -> bf16 -> global (b, s, h, d)
     l_a += __shfl_xor_sync(0xffffffffu, l_a, 1);

@@ -59,6 +59,12 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
 #ifndef AMB_WAIT_TIMEOUT_NS
 #define AMB_WAIT_TIMEOUT_NS 4000000000ull  // 4 s: a deadlocked pipeline traps instead of hanging the GPU
 #endif
+// Define AMB_WAIT_TIMEOUT_PRINT to 1 to print the block, thread and barrier of a timed-out wait before the trap.  Off by
+// default: printf is a function call, and any call in a kernel that issues wgmma makes ptxas serialize every wgmma in it
+// (C7510), which halves tensor throughput.
+#ifndef AMB_WAIT_TIMEOUT_PRINT
+#define AMB_WAIT_TIMEOUT_PRINT 0
+#endif
 // Bounded wait: a protocol bug becomes a trapped kernel (cudaErrorLaunchFailure), never a hung box.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
@@ -66,10 +72,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if ((++spins & 0xfff) == 0 && globaltimer_ns() - t0 > AMB_WAIT_TIMEOUT_NS) {
+#if AMB_WAIT_TIMEOUT_PRINT
       printf("amb: mbarrier wait timeout block=(%d,%d,%d) thread=%d bar=%u parity=%u\n", blockIdx.x, blockIdx.y,
              blockIdx.z, threadIdx.x, smem_u32(bar), parity);
+#endif
       __trap();
     }
+  }
+}
+// Unbounded wait, for warps whose progress another warp of the CTA watches with mbar_wait.  A trap in a warp that raised
+// its register budget with setmaxnreg caps what ptxas allocates there (about 176 registers instead of 240).
+__device__ __forceinline__ void mbar_wait_watched(uint64_t* bar, uint32_t parity) {
+  while (!mbar_try_wait(bar, parity)) {
   }
 }
 
@@ -183,6 +197,9 @@ __device__ __forceinline__ void wgmma_rs_n128_tb(float* d, const uint32_t* a, ui
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 template <int N>
