@@ -1,11 +1,19 @@
 // wgmma GEMM for sm_90a:  C = epilogue(A · Wᵀ),  A:(M,K) bf16, W:(N,K) bf16 (nn.Linear layout), fp32 accumulate in registers.
 //
-// One CTA computes one 128 x BN output tile; three warpgroups:
-//   warpgroup 0     TMA producer   (one elected lane; cp.async.bulk.tensor 2D, 128B swizzle, STAGES-deep mbarrier ring)
-//   warpgroups 1-2  consumers      (each owns 64 of the 128 rows: wgmma m64nBNk16 from shared memory, one k-block of MMAs
-//                                   in flight while the previous stage is released; then the epilogue straight from the
-//                                   accumulator fragment: bias / GELU / LayerScale / residual / per-head RMSNorm + RoPE)
-// Tiles are numbered n-fastest so the CTAs of one wave share A rows through L2 and W stays L2-resident.
+// Persistent, warp-specialized ping-pong kernel on 2-CTA clusters.  Output tiles are 128 x BN (BN = 128, or 64 when N is
+// not a multiple of 128).  The two CTAs of a cluster run tiles (m, n) and (m + 1, n) of one unit of the schedule together;
+// every CTA of a cluster runs the units cluster, cluster + clusters, ... in turn.  Three warpgroups per CTA:
+//   warpgroup 0     TMA producer   (one elected lane; cp.async.bulk.tensor 2D, 128B swizzle, STAGES-deep mbarrier ring).
+//                                  It loads its own A box and half of the W box, multicast into both CTAs of the pair, and
+//                                  runs ahead across tile boundaries so the ring never drains between tiles.
+//   warpgroups 1-2  consumers      (ping-pong: they take alternate tiles, each a whole 128 x BN tile = two wgmma m64nBNk16
+//                                   per k16 step, one k-block of MMAs in flight while the previous stage is released.
+//                                   Named barriers hand the tensor cores from one to the other after its last k-block, so
+//                                   one warpgroup's epilogue — bias / GELU / LayerScale / residual / per-head RMSNorm + RoPE
+//                                   straight from the accumulator fragment — runs under the other's MMAs.)
+// Units are rastered in bands of GROUP_M M-tile pairs: a band sweeps every N-tile before the next band starts, so its A
+// rows stay L2-resident while W panels stream past.
+#include <atomic>
 #include <cstdlib>
 #include "common.cuh"
 #include "ptx.cuh"
@@ -16,6 +24,9 @@ namespace amb {
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle-128B row
 constexpr int GEMM_THREADS = 384;
+constexpr int CLUSTER = 2;  // CTAs per cluster: M-tiles (m, m + 1) sharing each W box
+constexpr int GROUP_M = 8;    // M-tile pairs per raster band
+constexpr int EPI_BATCH = 4;  // column groups of residual loads in flight together (8 spills at 128 accumulator registers)
 
 struct GemmParams {
   int M, N, K;
@@ -61,7 +72,7 @@ __device__ __forceinline__ float gelu_erf(float x) {
 
 template <int BN>
 struct GemmSmem {
-  static constexpr int STAGES = BN == 256 ? 4 : BN == 128 ? 6 : 8;  // 192 KB of operand ring in every case
+  static constexpr int STAGES = BN == 128 ? 6 : 8;  // 192 KB of operand ring in both cases
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
@@ -79,8 +90,10 @@ __device__ __forceinline__ float2 load2(const void* R, int r_fp32, long long off
   return unpack_bf16(*reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(R) + off));
 }
 
-// bias -> activation -> column scale -> residual -> store for one (row, column pair)
-__device__ __forceinline__ void finish_pair(const GemmParams& p, float v0, float v1, long long drow, int col, bool valid) {
+// bias -> activation -> column scale -> residual -> store for one (row, column pair).  The residual r was loaded before
+// the stores of its batch (see epilogue_tile).
+__device__ __forceinline__ void finish_pair(const GemmParams& p, float v0, float v1, float2 r, long long drow, int col,
+                                            bool valid) {
   if (p.bias) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
     v0 += b.x; v1 += b.y;
@@ -94,16 +107,14 @@ __device__ __forceinline__ void finish_pair(const GemmParams& p, float v0, float
     v0 *= s.x; v1 *= s.y;
   }
   if (!valid) return;
-  if (p.residual) {
-    const float2 r = load2(p.residual, p.res_fp32, drow * p.ldr + col);
-    v0 += r.x; v1 += r.y;
-  }
+  if (p.residual) { v0 += r.x; v1 += r.y; }
   store2(p.C, p.c_fp32, drow * p.ldc + col, v0, v1);
   if (p.C2) store2(p.C2, 0, drow * p.ldc2 + col, v0, v1);
 }
 
-// Epilogue of one warpgroup's 64 x BN accumulator (fragment layout in ptx.cuh): thread holds rows r0 and r0 + 8, columns
-// 8i + 2q + {0,1}.  One head = 128 columns = 16 fragment groups; its row statistics are reduced over the 4 threads of a quad.
+// Epilogue of 64 rows of a 128 x BN accumulator (fragment layout in ptx.cuh): thread holds rows r0 and r0 + 8, columns
+// 8i + 2q + {0,1}.  A 128-column tile is one head (16 fragment groups); its row statistics are reduced over the 4 threads
+// of a quad.
 template <int BN>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* acc, int n0, int r0) {
   const int q = threadIdx.x & 3;
@@ -116,88 +127,108 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
     drow[h] = row[h];
     if (p.grp_rows > 0) drow[h] = (long long)(row[h] / p.grp_rows) * p.grp_stride + (row[h] % p.grp_rows) + p.row_off;
   }
-  const int head_cols = p.norm_cols > p.rope_cols ? p.norm_cols : p.rope_cols;
-  if constexpr (BN % 128 == 0) {
-    if (n0 < head_cols) {
+  if constexpr (BN == 128) {
+    const bool do_norm = n0 < p.norm_cols, do_rope = n0 < p.rope_cols;
+    if (do_norm || do_rope) {
       // ---- per-head RMSNorm and/or RoPE (the launch checks exclude residual / activation / col_scale / c2 here)
+      float rs[2] = {1.0f, 1.0f};
+      float2 nw[16];  // norm weights of my 16 column pairs
+      if (do_norm) {
+        const float* w = (n0 < p.norm_seg) ? p.norm_w0 : p.norm_w1;
 #pragma unroll
-      for (int hd = 0; hd < BN / 128; ++hd) {
-        const int col0 = n0 + hd * 128;
-        const bool do_norm = col0 < p.norm_cols, do_rope = col0 < p.rope_cols;
-        const float* a = acc + hd * 64;
-        if (!do_norm && !do_rope) {
+        for (int i = 0; i < 16; ++i) nw[i] = __ldg(reinterpret_cast<const float2*>(w + 8 * i + 2 * q));
+        float ss0 = 0.f, ss1 = 0.f;
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int col = col0 + 8 * i + 2 * q;
-            finish_pair(p, a[4 * i], a[4 * i + 1], drow[0], col, valid[0]);
-            finish_pair(p, a[4 * i + 2], a[4 * i + 3], drow[1], col, valid[1]);
-          }
-          continue;
+        for (int i = 0; i < 16; ++i) {
+          ss0 += acc[4 * i] * acc[4 * i] + acc[4 * i + 1] * acc[4 * i + 1];
+          ss1 += acc[4 * i + 2] * acc[4 * i + 2] + acc[4 * i + 3] * acc[4 * i + 3];
         }
-        float rs[2] = {1.0f, 1.0f};
-        if (do_norm) {
-          float ss0 = 0.f, ss1 = 0.f;
+        ss0 += __shfl_xor_sync(0xffffffffu, ss0, 1);
+        ss1 += __shfl_xor_sync(0xffffffffu, ss1, 1);
+        ss0 += __shfl_xor_sync(0xffffffffu, ss0, 2);
+        ss1 += __shfl_xor_sync(0xffffffffu, ss1, 2);
+        rs[0] = rsqrtf(ss0 * (1.0f / 128.0f) + p.norm_eps);
+        rs[1] = rsqrtf(ss1 * (1.0f / 128.0f) + p.norm_eps);
+      }
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            ss0 += a[4 * i] * a[4 * i] + a[4 * i + 1] * a[4 * i + 1];
-            ss1 += a[4 * i + 2] * a[4 * i + 2] + a[4 * i + 3] * a[4 * i + 3];
-          }
-          ss0 += __shfl_xor_sync(0xffffffffu, ss0, 1);
-          ss1 += __shfl_xor_sync(0xffffffffu, ss1, 1);
-          ss0 += __shfl_xor_sync(0xffffffffu, ss0, 2);
-          ss1 += __shfl_xor_sync(0xffffffffu, ss1, 2);
-          rs[0] = rsqrtf(ss0 * (1.0f / 128.0f) + p.norm_eps);
-          rs[1] = rsqrtf(ss1 * (1.0f / 128.0f) + p.norm_eps);
-        }
-        const float* w = (col0 < p.norm_seg) ? p.norm_w0 : p.norm_w1;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
+      for (int h = 0; h < 2; ++h) {
+        float rc[16], rsn[16];  // RoPE cos / sin of my 16 pairs at this row's position
+        if (do_rope) {
           const int pos = (valid[h] ? row[h] : 0) / p.rope_rows_per_pos;
           const float* cs = p.rope_cos + (long long)pos * 64;
           const float* sn = p.rope_sin + (long long)pos * 64;
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
-            const int lc = 8 * i + 2 * q;  // column inside the head
-            float v0 = a[4 * i + 2 * h], v1 = a[4 * i + 2 * h + 1];
-            if (do_norm) {
-              const float2 ww = __ldg(reinterpret_cast<const float2*>(w + lc));
-              v0 *= rs[h] * ww.x;
-              v1 *= rs[h] * ww.y;
-            }
-            if (do_rope) {  // interleaved pair (lc, lc + 1) rotates by angle lc / 2 of the row's position
-              const float c = __ldg(cs + (lc >> 1)), s = __ldg(sn + (lc >> 1));
-              const float x = v0, y = v1;
-              v0 = x * c - y * s;
-              v1 = y * c + x * s;
-            }
-            if (valid[h]) store2(p.C, p.c_fp32, drow[h] * p.ldc + col0 + lc, v0, v1);
+            rc[i] = __ldg(cs + 4 * i + q);  // angle index lc / 2 of column lc = 8i + 2q
+            rsn[i] = __ldg(sn + 4 * i + q);
           }
+        }
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int lc = 8 * i + 2 * q;  // column inside the head
+          float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+          if (do_norm) {
+            v0 *= rs[h] * nw[i].x;
+            v1 *= rs[h] * nw[i].y;
+          }
+          if (do_rope) {  // interleaved pair (lc, lc + 1) rotates by angle lc / 2 of the row's position
+            const float c = rc[i], s = rsn[i];
+            const float x = v0, y = v1;
+            v0 = x * c - y * s;
+            v1 = y * c + x * s;
+          }
+          if (valid[h]) store2(p.C, p.c_fp32, drow[h] * p.ldc + n0 + lc, v0, v1);
         }
       }
       return;
     }
   }
+  // The residual may alias C, so a residual load placed after a store cannot move above it: loaded pair by pair, every
+  // load of the tile would wait out a full HBM latency behind the previous pair's stores.  Instead the residuals of EPI_BATCH
+  // column groups are loaded together, before any of their stores.
 #pragma unroll
-  for (int i = 0; i < BN / 8; ++i) {
-    const int col = n0 + 8 * i + 2 * q;
-    finish_pair(p, acc[4 * i], acc[4 * i + 1], drow[0], col, valid[0]);
-    finish_pair(p, acc[4 * i + 2], acc[4 * i + 3], drow[1], col, valid[1]);
+  for (int i0 = 0; i0 < BN / 8; i0 += EPI_BATCH) {
+    float2 r[EPI_BATCH][2];
+#pragma unroll
+    for (int i = 0; i < EPI_BATCH; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        r[i][h] = (p.residual && valid[h]) ? load2(p.residual, p.res_fp32, drow[h] * p.ldr + n0 + 8 * (i0 + i) + 2 * q)
+                                           : make_float2(0.f, 0.f);
+#pragma unroll
+    for (int i = 0; i < EPI_BATCH; ++i) {
+      const int col = n0 + 8 * (i0 + i) + 2 * q;
+      const float* a = acc + 4 * (i0 + i);
+      finish_pair(p, a[0], a[1], r[i][0], drow[0], col, valid[0]);
+      finish_pair(p, a[2], a[3], r[i][1], drow[1], col, valid[1]);
+    }
   }
 }
 
 template <int BN>
 __device__ __forceinline__ void wgmma_tile_k16(float* acc, uint64_t adesc, uint64_t bdesc) {
-  if constexpr (BN == 256) wgmma_ss_n256(acc, adesc, bdesc, 1u);
-  else if constexpr (BN == 128) wgmma_ss_n128(acc, adesc, bdesc, 1u);
+  if constexpr (BN == 128) wgmma_ss_n128(acc, adesc, bdesc, 1u);
   else wgmma_ss_n64(acc, adesc, bdesc, 1u);
 }
 
+// First row m0 and N-tile index nt of schedule unit u for cluster CTA `rank`: bands of GROUP_M M-tile pairs, the M pair
+// fastest inside a band.
+__device__ __forceinline__ void unit_tile(int u, int num_mp, int num_n, uint32_t rank, int& m0, int& nt) {
+  const int band = u / (GROUP_M * num_n);
+  const int first = band * GROUP_M;
+  const int rows = min(GROUP_M, num_mp - first);
+  const int r = u - band * GROUP_M * num_n;
+  m0 = ((first + r % rows) * CLUSTER + (int)rank) * BM;
+  nt = r / rows;
+}
+
 template <int BN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                  const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using L = GemmSmem<BN>;
   constexpr int STAGES = L::STAGES;
+  constexpr int B_HALF = L::B_BYTES / CLUSTER;  // the W rows one CTA loads for the pair: a whole number of 1024-B swizzle atoms
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
@@ -206,21 +237,23 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);  // warp-uniform role
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const uint32_t rank = cluster_ctarank();
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmA2);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
+      mbar_init(&empty_bar[s], 4 * CLUSTER);  // one arrival per consumer warp of both CTAs: each wrote a W half here
     }
     fence_mbar_init();
   }
-  __syncthreads();
+  cluster_sync();  // both CTAs' barriers exist before any multicast copy or remote arrival reaches them
 
-  const int num_n_tiles = p.N / BN;
-  const int m0 = (blockIdx.x / num_n_tiles) * BM;
-  const int n0 = (blockIdx.x % num_n_tiles) * BN;
+  const int num_n = p.N / BN;
+  const int num_mp = (p.M + CLUSTER * BM - 1) / (CLUSTER * BM);  // M-tile pairs; the odd last tile's peer has no valid row
+  const int num_units = num_mp * num_n;
+  const int cluster = blockIdx.x / CLUSTER, num_clusters = gridDim.x / CLUSTER;
   const int num_kb = p.K / BK;
 
   if (wg == 0) {
@@ -229,52 +262,91 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (warp == 0) {
       int s = 0;
       uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[s], phase ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&full_bar[s], L::STAGE_BYTES);
-          uint8_t* sa = smem + s * L::STAGE_BYTES;
-          uint8_t* sb = sa + L::A_BYTES;
-          if (kb < p.k_split_blocks) tma_load_2d(sa, &tmA, &full_bar[s], kb * BK, m0, kEvictNormal);
-          else tma_load_2d(sa, &tmA2, &full_bar[s], (kb - p.k_split_blocks) * BK, m0, kEvictNormal);
-          tma_load_2d(sb, &tmB, &full_bar[s], kb * BK, n0, kEvictLast);
+      for (int u = cluster; u < num_units; u += num_clusters) {
+        int m0, nt;
+        unit_tile(u, num_mp, num_n, rank, m0, nt);
+        const int n0 = nt * BN;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[s], phase ^ 1);  // released by the consumers of both CTAs
+          if (elect_one()) {
+            mbar_expect_tx(&full_bar[s], L::STAGE_BYTES);
+            uint8_t* sa = smem + s * L::STAGE_BYTES;
+            uint8_t* sb = sa + L::A_BYTES;
+            if (kb < p.k_split_blocks) tma_load_2d(sa, &tmA, &full_bar[s], kb * BK, m0, kEvictNormal);
+            else tma_load_2d(sa, &tmA2, &full_bar[s], (kb - p.k_split_blocks) * BK, m0, kEvictNormal);
+            tma_load_2d_multicast(sb + rank * B_HALF, &tmB, &full_bar[s], kb * BK, n0 + (int)rank * (BN / CLUSTER),
+                                  (uint16_t)((1u << CLUSTER) - 1), kEvictLast);
+          }
+          __syncwarp();
+          if (++s == STAGES) { s = 0; phase ^= 1; }
         }
-        __syncwarp();
+      }
+      // Watchdog: the consumers wait without a timeout (see mbar_wait_watched), so this warp waits, bounded, until they
+      // have released the last STAGES stages.  A stalled consumer makes that wait trap and the launch fail.
+      for (int j = 0; j < STAGES; ++j) {
+        mbar_wait(&empty_bar[s], phase ^ 1);
         if (++s == STAGES) { s = 0; phase ^= 1; }
       }
     }
   } else {
-    // ===================== consumers: warpgroup 1 rows [0, 64), warpgroup 2 rows [64, 128) of the tile =====================
+    // ===================== consumers: warpgroup 1 takes this CTA's even tiles, warpgroup 2 its odd ones =====================
     reg_alloc<232>();
-    float acc[BN / 2];
+    // Issue turns: a warpgroup waits on named barrier `wg` before its mainloop and lets the other one go after issuing its
+    // last k-block.  The first tile goes without waiting and the last gives no go-ahead, so every arrival meets a wait.
+    const uint32_t my_turn = wg, other_turn = 3 - wg;
+    const int n_local = (num_units - cluster + num_clusters - 1) / num_clusters;
+    for (int i = wg - 1; i < n_local; i += 2) {
+      int m0, nt;
+      unit_tile(cluster + i * num_clusters, num_mp, num_n, rank, m0, nt);
+      const int n0 = nt * BN;
+      float acc[2][BN / 2];  // rows [0, 64) and [64, 128) of the tile
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    const uint32_t a_row_off = (wg - 1) * 64 * 128;  // 64 rows of 128 B (a multiple of the 1024-B swizzle atom)
-    int s = 0, s_prev = 0;
-    uint32_t phase = 0;
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full_bar[s], phase);
-      const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
-      const uint64_t adesc = make_desc_kmajor_sw128(a_addr + a_row_off);
-      const uint64_t bdesc = make_desc_kmajor_sw128(a_addr + L::A_BYTES);
-      wgmma_fence();
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) wgmma_tile_k16<BN>(acc, adesc + 2 * k, bdesc + 2 * k);
-      wgmma_commit();
-      wgmma_wait<1>();  // the MMAs of the previous k-block are complete: its stage can be refilled
-      if (kb > 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[s_prev]);
+        for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
+      // the producer filled the ring in tile order: this tile's first k-block is ring slot i * num_kb
+      const long long g0 = (long long)i * num_kb;
+      int s = (int)(g0 % STAGES), s_prev = s;
+      uint32_t phase = (uint32_t)((g0 / STAGES) & 1);
+      if (i > 0) named_bar_sync(my_turn, 256);
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait_watched(&full_bar[s], phase);
+        const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
+        const uint64_t adesc0 = make_desc_kmajor_sw128(a_addr);
+        const uint64_t adesc1 = make_desc_kmajor_sw128(a_addr + 64 * 128);  // 64 rows of 128 B
+        const uint64_t bdesc = make_desc_kmajor_sw128(a_addr + L::A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          wgmma_tile_k16<BN>(acc[0], adesc0 + 2 * k, bdesc + 2 * k);
+          wgmma_tile_k16<BN>(acc[1], adesc1 + 2 * k, bdesc + 2 * k);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the MMAs of the previous k-block are complete: its stage can be refilled
+        if (kb > 0) {
+          __syncwarp();
+          if (lane < CLUSTER) mbar_arrive_cluster(&empty_bar[s_prev], lane);  // lane c releases the stage in CTA c
+        }
+        s_prev = s;
+        if (++s == STAGES) { s = 0; phase ^= 1; }
       }
-      s_prev = s;
-      if (++s == STAGES) { s = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
+      if (i + 1 < n_local) named_bar_arrive(other_turn, 256);
+      wgmma_wait<0>();
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
-    const int r0 = m0 + (wg - 1) * 64 + (warp & 3) * 16 + (lane >> 2);
-    epilogue_tile<BN>(p, acc, n0, r0);
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) reg_fence(acc[h][j]);
+      __syncwarp();
+      if (lane < CLUSTER) mbar_arrive_cluster(&empty_bar[s_prev], lane);
+      if (m0 < p.M) {
+        const int r0 = m0 + (warp & 3) * 16 + (lane >> 2);
+        epilogue_tile<BN>(p, acc[0], n0, r0);
+        epilogue_tile<BN>(p, acc[1], n0, r0 + 64);
+      }
+    }
   }
+  __syncwarp();
+  cluster_sync();  // no CTA leaves while its peer can still write into its shared memory or arrive on its barriers
 }
 
 static GemmParams make_params(const amb_gemm_args* a) {
@@ -294,6 +366,29 @@ static GemmParams make_params(const amb_gemm_args* a) {
   p.rope_rows_per_pos = a->rope_rows_per_pos > 0 ? a->rope_rows_per_pos : 1;
   p.C2 = a->c2; p.ldc2 = a->ldc2;
   return p;
+}
+
+// Clusters of gemm_bf16_kernel<BN> that fit on the current device at once, queried once per device: the persistent grid
+// never launches more, so no cluster waits for a second wave.
+template <int BN>
+static int max_active_clusters(int* out) {
+  static std::atomic<int> cached[16];
+  int dev = 0;
+  AMB_CHECK_CUDA(cudaGetDevice(&dev));
+  if (dev < 16 && cached[dev].load() > 0) {
+    *out = cached[dev].load();
+    return AMB_OK;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(CLUSTER * num_sms(), 1, 1);
+  cfg.blockDim = dim3(GEMM_THREADS, 1, 1);
+  cfg.dynamicSmemBytes = GemmSmem<BN>::TOTAL;
+  int n = 0;
+  AMB_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, gemm_bf16_kernel<BN>, &cfg));
+  AMB_CHECK_ARG(n > 0, "gemm: no %d-CTA cluster of %d B shared memory fits on device %d", CLUSTER, GemmSmem<BN>::TOTAL, dev);
+  if (dev < 16) cached[dev].store(n);
+  *out = n;
+  return AMB_OK;
 }
 
 template <int BN>
@@ -320,7 +415,7 @@ static int launch_gemm(const amb_gemm_args* a, cudaStream_t stream) {
   {
     uint64_t dims[2] = {(uint64_t)a->k, (uint64_t)a->n};
     uint64_t str[1] = {(uint64_t)a->ldw * 2};
-    uint32_t box[2] = {BK, BN};
+    uint32_t box[2] = {BK, BN / CLUSTER};  // each CTA of a pair loads half of the W tile
     int r = encode_tmap_bf16(&tmB, a->w, 2, dims, str, box);
     if (r) return r;
   }
@@ -330,9 +425,16 @@ static int launch_gemm(const amb_gemm_args* a, cudaStream_t stream) {
     int r = ensure_smem_optin(kern, L::TOTAL);
     if (r) return r;
   }
-  const long long num_tiles = (long long)(a->n / BN) * ((a->m + BM - 1) / BM);
-  AMB_CHECK_ARG(num_tiles < 0x7fffffffLL, "gemm: too many tiles (m=%d n=%d)", a->m, a->n);
-  kern<<<(unsigned)num_tiles, GEMM_THREADS, L::TOTAL, stream>>>(tmA, tmA2, tmB, p);
+  int clusters = 0;
+  {
+    int r = max_active_clusters<BN>(&clusters);
+    if (r) return r;
+  }
+  const long long num_mp = ((long long)a->m + CLUSTER * BM - 1) / (CLUSTER * BM);
+  const long long num_units = (long long)(a->n / BN) * num_mp;
+  AMB_CHECK_ARG(num_units < 0x7fffffffLL, "gemm: too many tiles (m=%d n=%d)", a->m, a->n);
+  const unsigned grid = (unsigned)(CLUSTER * (num_units < clusters ? num_units : clusters));
+  kern<<<grid, GEMM_THREADS, L::TOTAL, stream>>>(tmA, tmA2, tmB, p);
   AMB_CHECK_CUDA(cudaGetLastError());
   return AMB_OK;
 }
@@ -360,7 +462,6 @@ extern "C" int amb_gemm_bf16(const amb_gemm_args* a, amb_stream_t stream) {
     AMB_CHECK_ARG(!a->residual && a->act == 0 && !a->col_scale && !a->c2, "gemm: head epilogue excludes residual/activation/col_scale/c2");
   }
   cudaStream_t s = (cudaStream_t)stream;
-  if (a->n % 256 == 0) return launch_gemm<256>(a, s);
   if (a->n % 128 == 0) return launch_gemm<128>(a, s);
   return launch_gemm<64>(a, s);
 }

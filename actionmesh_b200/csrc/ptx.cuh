@@ -51,6 +51,28 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity
       : "memory");
   return ok;
 }
+// Arrive on the barrier at bar's shared-memory offset in cluster CTA `cta` (which may be this CTA).  Default .release.cta
+// semantics: it releases stage reads already completed by wgmma.wait_group, not writes.  A .cluster-scope release would
+// compile to MEMBAR.ALL.GPU and wait for every global store still in flight (e.g. the previous tile's epilogue).
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}\n"
+      ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
+}
+
+// ------------------------------------------------------------------ thread-block cluster
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// Every thread of every CTA in the cluster: release what it wrote (barrier init included), acquire the others'.
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 __device__ __forceinline__ uint64_t globaltimer_ns() {
   uint64_t t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -103,6 +125,18 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const void* tmap, uint64_
       " [%0], [%1, {%3, %4}], [%2], %5;"
       :
       : "r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
+      : "memory");
+}
+// The same box delivered to the same shared-memory offset of every CTA in cta_mask; each destination CTA's barrier at
+// bar's offset receives the complete_tx of its copy.
+__device__ __forceinline__ void tma_load_2d_multicast(void* dst, const void* tmap, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask, uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%4, %5}], [%2], %3, %6;"
+      :
+      : "r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0), "r"(c1),
+        "l"(hint)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_4d(void* dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2,

@@ -205,6 +205,15 @@ def group_gemm(res):
     _gemm_case(res, "g_norm_kv_bias", 300, 512, 128, norm=(256, 256, 0, 1), bias=True)
 
 
+def _cublas_case(res, m, n, k):
+    """torch.matmul (cuBLAS) on the same bf16 shape, bf16 out and no epilogue: a measured ceiling beside our number."""
+    import torch
+    a = torch.randn(m, k, device="cuda").bfloat16()
+    w = torch.randn(n, k, device="cuda").bfloat16()
+    ms = _time(lambda: torch.matmul(a, w.t()), iters=5)
+    res[f"cublas_{m}x{n}x{k}"] = {"ms": ms, "TFLOPs": 2.0 * m * n * k / ms / 1e9}
+
+
 def group_gemm_perf(res):
     _gemm_case(res, "p_8192x2048x2048", 8192, 2048, 2048, timing=True)
     _gemm_case(res, "p_65568x2048x2048_res", 65568, 2048, 2048, bias=True, residual=True, timing=True)
@@ -212,12 +221,9 @@ def group_gemm_perf(res):
     _gemm_case(res, "p_65568x2048x8192_res", 65568, 2048, 8192, bias=True, residual=True, timing=True)
     _gemm_case(res, "p_65568x6144x2048_qkv", 65568, 6144, 2048, norm=(4096, 2048, 4096, 2049), timing=True)
     _gemm_case(res, "p_65568x2048x4096_skip", 65568, 2048, 4096, a2=True, bias=True, timing=True)
-    import torch
-    # cuBLAS reference point for the same shape (baseline only)
-    a = torch.randn(65568, 2048, device="cuda").bfloat16()
-    w = torch.randn(2048, 2048, device="cuda").bfloat16()
-    ms = _time(lambda: torch.matmul(a, w.t()), iters=5)
-    res["cublas_65568x2048x2048"] = {"ms": ms, "TFLOPs": 2.0 * 65568 * 2048 * 2048 / ms / 1e9}
+    for m, n, k in ((8192, 2048, 2048), (65568, 2048, 2048), (65568, 8192, 2048), (65568, 2048, 8192),
+                    (65568, 6144, 2048), (65568, 2048, 4096)):
+        _cublas_case(res, m, n, k)
 
 
 def _attn_ref(q, k, v, scale):
