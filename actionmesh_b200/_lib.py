@@ -10,12 +10,15 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libactionmesh_b200.so")
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 
 EXPORTS = [
     "amb_last_error", "amb_abi_version", "amb_device_info", "amb_cfg_euler_step", "amb_layernorm",
     "amb_cast_f32_bf16", "amb_patchify", "amb_timestep_embedding", "amb_alpha_rows", "amb_point_embedding",
     "amb_displacement_out", "amb_split3_bf16", "amb_softmax_split3", "amb_resize_h_u8", "amb_resize_v_normalize", "amb_alpha_stats", "amb_composite_crop_pad", "amb_nearest_neighbors", "amb_add_bias_rows", "amb_gemm_bf16", "amb_flash_attn_fwd", "amb_attn_small_f32",
+    "amb_scan_scratch_ints", "amb_octree_near_surface", "amb_octree_dilate", "amb_octree_mark_upsampled",
+    "amb_octree_count_points", "amb_octree_emit_points", "amb_grid_fill", "amb_grid_replace", "amb_grid_scatter",
+    "amb_dmc_count", "amb_dmc_emit",
 ]
 
 
@@ -105,6 +108,19 @@ def load_library() -> C.CDLL:
     lib.amb_flash_attn_fwd.argtypes = [C.POINTER(AttnArgs), C.c_void_p]
     lib.amb_attn_small_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_float,
                                        C.c_void_p, C.c_int64, C.c_void_p]
+    lib.amb_scan_scratch_ints.argtypes = [C.c_int64, C.POINTER(C.c_int64)]
+    lib.amb_octree_near_surface.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.amb_octree_dilate.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.amb_octree_mark_upsampled.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.amb_octree_count_points.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.amb_octree_emit_points.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                           C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.amb_grid_fill.argtypes = [C.c_void_p, C.c_int64, C.c_float, C.c_void_p]
+    lib.amb_grid_replace.argtypes = [C.c_void_p, C.c_int64, C.c_float, C.c_float, C.c_void_p]
+    lib.amb_grid_scatter.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.amb_dmc_count.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.amb_dmc_emit.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if name != "amb_last_error":

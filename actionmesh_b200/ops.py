@@ -457,3 +457,121 @@ def flash_attn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Ten
     _lib.check(rc, "amb_flash_attn_fwd")
     launch_count += 1
     return out
+
+
+# ---- Stage 0's anchor mesh: octree refinement + dual marching cubes (csrc/geometry.cu) --------------------------------------
+def _scan_scratch(n_items: int, device) -> torch.Tensor:
+    nints = C.c_int64()
+    _lib.check(_lib.load_library().amb_scan_scratch_ints(int(n_items), C.byref(nints)), "amb_scan_scratch_ints")
+    return torch.empty(nints.value, dtype=torch.int32, device=device)
+
+
+def _cube(t: torch.Tensor, dtype: torch.dtype, name: str) -> int:
+    _need(t, dtype, name)
+    assert t.dim() == 3 and t.shape[0] == t.shape[1] == t.shape[2] and t.is_contiguous(), f"{name}: expected a contiguous cube"
+    return t.shape[0]
+
+
+def octree_near_surface(grid: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """(n,n,n) fp32 logits -> uint8 mask of the near-surface band (sign change to a face neighbour, or |logit| < 0.95)."""
+    global launch_count
+    n = _cube(grid, torch.float32, "grid")
+    out = torch.empty_like(grid, dtype=torch.uint8) if out is None else out
+    _cube(out, torch.uint8, "out")
+    _lib.check(_lib.load_library().amb_octree_near_surface(grid.data_ptr(), n, out.data_ptr(), _stream()), "amb_octree_near_surface")
+    launch_count += 1
+    return out
+
+
+def octree_dilate(mask: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """3x3x3 zero-padded dilation of a uint8 mask (out must not alias mask)."""
+    global launch_count
+    n = _cube(mask, torch.uint8, "mask")
+    out = torch.empty_like(mask) if out is None else out
+    _cube(out, torch.uint8, "out")
+    _lib.check(_lib.load_library().amb_octree_dilate(mask.data_ptr(), n, out.data_ptr(), _stream()), "amb_octree_dilate")
+    launch_count += 1
+    return out
+
+
+def octree_mark_upsampled(mask: torch.Tensor) -> torch.Tensor:
+    """(n,n,n) uint8 -> (2n-1)^3 uint8 with fine[2x, 2y, 2z] = mask[x, y, z] and zeros elsewhere."""
+    global launch_count
+    n = _cube(mask, torch.uint8, "mask")
+    fine = torch.empty((2 * n - 1,) * 3, dtype=torch.uint8, device=mask.device)
+    _lib.check(_lib.load_library().amb_octree_mark_upsampled(mask.data_ptr(), n, fine.data_ptr(), _stream()),
+               "amb_octree_mark_upsampled")
+    launch_count += 2
+    return fine
+
+
+def octree_points(mask: torch.Tensor, resolution, bbox_min) -> tuple[torch.Tensor, torch.Tensor]:
+    """Set cells of a uint8 mask in grid order -> (xyz (P, 3) fp32 = fp32(idx) * resolution + bbox_min, linear index (P,) int32).
+    Reads P back to the host (one sync)."""
+    global launch_count
+    n = _cube(mask, torch.uint8, "mask")
+    lib = _lib.load_library()
+    scratch = _scan_scratch(n ** 3, mask.device)
+    _lib.check(lib.amb_octree_count_points(mask.data_ptr(), n, scratch.data_ptr(), _stream()), "amb_octree_count_points")
+    count = int(scratch[-1].item())
+    xyz = torch.empty(count, 3, dtype=torch.float32, device=mask.device)
+    index = torch.empty(count, dtype=torch.int32, device=mask.device)
+    res = (C.c_float * 3)(*[float(v) for v in resolution])
+    lo = (C.c_float * 3)(*[float(v) for v in bbox_min])
+    if count:
+        _lib.check(lib.amb_octree_emit_points(mask.data_ptr(), n, scratch.data_ptr(), res, lo, xyz.data_ptr(), index.data_ptr(),
+                                              _stream()), "amb_octree_emit_points")
+    launch_count += 4
+    return xyz, index
+
+
+def grid_fill(grid: torch.Tensor, value: float) -> torch.Tensor:
+    global launch_count
+    _need(grid, torch.float32, "grid")
+    assert grid.is_contiguous()
+    _lib.check(_lib.load_library().amb_grid_fill(grid.data_ptr(), grid.numel(), float(value), _stream()), "amb_grid_fill")
+    launch_count += 1
+    return grid
+
+
+def grid_replace(grid: torch.Tensor, value_from: float, value_to: float) -> torch.Tensor:
+    global launch_count
+    _need(grid, torch.float32, "grid")
+    assert grid.is_contiguous()
+    _lib.check(_lib.load_library().amb_grid_replace(grid.data_ptr(), grid.numel(), float(value_from), float(value_to), _stream()),
+               "amb_grid_replace")
+    launch_count += 1
+    return grid
+
+
+def grid_scatter(values: torch.Tensor, index: torch.Tensor, grid: torch.Tensor) -> torch.Tensor:
+    """grid.view(-1)[index[i]] = values[i, 0] for fp32 `values` (P, k) with any row stride."""
+    global launch_count
+    _need(values, torch.float32, "values")
+    _need(index, torch.int32, "index")
+    _need(grid, torch.float32, "grid")
+    assert values.dim() == 2 and values.shape[0] == index.numel() and index.is_contiguous() and grid.is_contiguous()
+    _lib.check(_lib.load_library().amb_grid_scatter(values.data_ptr(), values.stride(0), index.data_ptr(), index.numel(),
+                                                    grid.data_ptr(), _stream()), "amb_grid_scatter")
+    launch_count += 1
+    return grid
+
+
+def dual_marching_cubes(grid: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Dual marching cubes of the zero level set of an (n,n,n) fp32 grid (inside = value > 0; non-finite cells emit nothing)
+    -> vertices (V, 3) fp32 in grid-index units, faces (F, 3) int32 wound outward.  Reads V and F back (one sync)."""
+    global launch_count
+    n = _cube(grid, torch.float32, "grid")
+    lib = _lib.load_library()
+    dev = grid.device
+    cases = torch.empty((n - 1,) * 3, dtype=torch.uint8, device=dev)
+    vs, fs = _scan_scratch((n - 1) ** 3, dev), _scan_scratch(n ** 3, dev)
+    _lib.check(lib.amb_dmc_count(grid.data_ptr(), n, cases.data_ptr(), vs.data_ptr(), fs.data_ptr(), _stream()), "amb_dmc_count")
+    nv, nf = (int(v) for v in torch.stack([vs[-1], fs[-1]]).tolist())
+    voff = torch.empty((n - 1,) * 3, dtype=torch.int32, device=dev)
+    verts = torch.empty(max(nv, 1), 3, dtype=torch.float32, device=dev)
+    faces = torch.empty(max(nf, 1), 3, dtype=torch.int32, device=dev)
+    _lib.check(lib.amb_dmc_emit(grid.data_ptr(), n, cases.data_ptr(), vs.data_ptr(), fs.data_ptr(), voff.data_ptr(),
+                                verts.data_ptr(), faces.data_ptr(), _stream()), "amb_dmc_emit")
+    launch_count += 9
+    return verts[:nv], faces[:nf]

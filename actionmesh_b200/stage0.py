@@ -13,8 +13,9 @@ to its bias (SURVEY A.5).
 Precision: the reference runs this stage in fp16 (pipeline.py:142); here GEMM / attention operands are bf16 with fp32
 accumulation and an fp32 residual stream, latents stay fp32 between steps (the reference rounds them to fp16 every step,
 scheduling_rectified_flow.py:299).  tests/test_stage0_gpu.py states the tolerance against the fp32 reference modules.
-The VAE decoder / iso-surface extraction that turn the latent into the anchor MESH (diso, flash decoder) are not part of
-this package: `TripoSGStage0` takes them as an injected callable.
+The VAE decoder and the iso-surface extraction that turn the latent into the anchor MESH live in triposg_vae.py:
+`TripoSGStage0(..., mesh_extractor=B200TripoSGVAE.extract_mesh)` (bound to a loaded VAE).  Without an extractor,
+`__call__` raises.
 """
 from __future__ import annotations
 
@@ -132,7 +133,7 @@ class TripoSGStage0:
     (anchor_latent (1, N, C) fp32, anchor_mesh), as `TripoSGPipelinePlus.__call__` (actionmesh/external/triposg.py:35).
 
     `image_encoder`: B200ImageEncoder with TripoSG's DinoV2 weights (pipeline_triposg.py:137-145); `mesh_extractor(latents)`:
-    the VAE decode + iso-surface extraction (out of scope; injected)."""
+    the VAE decode + iso-surface extraction, e.g. `B200TripoSGVAE(...).extract_mesh` (triposg_vae.py)."""
 
     def __init__(self, transformer: B200TripoSGDiT, image_encoder, mesh_extractor: Optional[Callable] = None,
                  shift: float = 1.0, num_tokens: int = 2048):

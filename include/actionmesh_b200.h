@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define AMB_ABI_VERSION 14
+#define AMB_ABI_VERSION 15
 
 typedef void* amb_stream_t; /* cudaStream_t */
 
@@ -209,6 +209,39 @@ int amb_flash_attn_fwd(const amb_attn_args* args, amb_stream_t stream);
  * seq <= 320.  No mask, non-causal; softmax(scale * q k^T) v with fp32 arithmetic throughout (CUDA cores). */
 int amb_attn_small_f32(const float* q, const float* k, const float* v, int64_t ld, int frames, int seq, int heads, float scale,
                        float* out, int64_t ldo, amb_stream_t stream);
+
+/* ---- Stage 0's anchor mesh: octree refinement + dual marching cubes (SURVEY 8(f) row f2) ------------------------------
+ * Replaces flash_extract_geometry (third_party/TripoSG/triposg/inference_utils.py:318-479) after the decoder calls, and the
+ * DiffDMC iso-surface extraction it hands the final grid to.  Grids are cubic with n points per side, x slowest:
+ * element (x, y, z) at (x * n + y) * n + z.  Masks are uint8 0/1.
+ *  octree_near_surface: mask = (a face neighbour has another sign, with replicate padding and invalid (<= -9000) neighbours
+ *    replaced by the cell itself, on a valid cell) or |logit| < 0.95 (inference_utils.py:203-297,402-403).
+ *  octree_dilate: out = any of the 3x3x3 zero-padded neighbourhood set (the ones-Conv3d "> 0" of :361-362,410-416).
+ *  octree_mark_upsampled: fine ((2n-1)^3) = 0 except fine[2x, 2y, 2z] = coarse[x, y, z] (:414).
+ *  octree_count_points / octree_emit_points: the set cells of a mask as a point list in grid order, xyz fp32 (P, 3) =
+ *    fp32(idx) * resolution + bbox_min with both ops rounded separately (:417-421; resolution and bbox_min are HOST
+ *    pointers to 3 floats) and the linear grid index (P).  `scratch` holds amb_scan_scratch_ints(n^3) ints; after the
+ *    count, its last entry (device memory) is P.
+ *  grid_fill / grid_replace / grid_scatter: g[:] = value; g[g == from] = to; g[index[i]] = values[i * ld].
+ *  dmc_count / dmc_emit: dual marching cubes of the zero level set, inside = logit > 0.  cases: (n-1)^3 bytes;
+ *    vertex_scratch: amb_scan_scratch_ints((n-1)^3) ints, face_scratch: amb_scan_scratch_ints(n^3) ints; after the count
+ *    their last entries are V and F.  dmc_emit writes vertex_offsets ((n-1)^3 int32), vertices (V, 3) fp32 in grid-index
+ *    units, faces (F, 3) int32 wound outward from the inside.  The patch table and the face rules are in csrc/geometry.cu
+ *    and DESIGN.md. */
+int amb_scan_scratch_ints(int64_t n_items, int64_t* out_ints);
+int amb_octree_near_surface(const float* grid, int n, uint8_t* mask, amb_stream_t stream);
+int amb_octree_dilate(const uint8_t* in, int n, uint8_t* out, amb_stream_t stream);
+int amb_octree_mark_upsampled(const uint8_t* coarse, int n, uint8_t* fine, amb_stream_t stream);
+int amb_octree_count_points(const uint8_t* mask, int n, int32_t* scratch, amb_stream_t stream);
+int amb_octree_emit_points(const uint8_t* mask, int n, const int32_t* scratch, const float* resolution3_host,
+                           const float* bbox_min3_host, float* xyz, int32_t* index, amb_stream_t stream);
+int amb_grid_fill(float* grid, int64_t count, float value, amb_stream_t stream);
+int amb_grid_replace(float* grid, int64_t count, float from, float to, amb_stream_t stream);
+int amb_grid_scatter(const float* values, int64_t ld, const int32_t* index, int count, float* grid, amb_stream_t stream);
+int amb_dmc_count(const float* grid, int n, uint8_t* cases, int32_t* vertex_scratch, int32_t* face_scratch,
+                  amb_stream_t stream);
+int amb_dmc_emit(const float* grid, int n, const uint8_t* cases, const int32_t* vertex_scratch, const int32_t* face_scratch,
+                 int32_t* vertex_offsets, float* vertices, int32_t* faces, amb_stream_t stream);
 
 #ifdef __cplusplus
 }

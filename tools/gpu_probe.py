@@ -341,9 +341,74 @@ def group_attn_more(res):
     res["am_late_rescale"] = _err(o, _attn_ref(q, k, v, 1 / math.sqrt(D)))
 
 
+def _card():
+    import torch
+    try:
+        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                             str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception:  # noqa: BLE001
+        pl = "unknown"
+    return {"name": torch.cuda.get_device_name(), "power_limit": pl}
+
+
+def group_vae_decode(res):
+    """TripoSG VAE decode + anchor-mesh extraction at full width (1024, 8 heads, 16 layers, 2048 latent tokens).
+    TFLOP/s of the query path from the shape count: q-proj 2D^2 + attention 4 Sk D + o-proj 2D^2 + FF 16 D^2 per point."""
+    import torch
+
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import triposg_vae_ref as ref
+    from actionmesh_b200.triposg_vae import B200TripoSGVAE, mesh_from_grid, refine_octree
+
+    res["card"] = _card()
+    D, Sk = 1024, 2048
+    sd = ref.make_state_dict(D, 8, 16, seed=1)
+    vae = B200TripoSGVAE().to("cuda")
+    vae.load_state_dict(sd)
+    g = torch.Generator(device="cuda").manual_seed(0)
+    z = torch.randn(2048, 64, device="cuda", generator=g)
+    ctx = vae.prepare(z)
+    res["trunk_kv_ms"] = {"ms": _time(lambda: vae.prepare(z), iters=5)}
+    flop_pt = 2 * D * D + 4 * Sk * D + 2 * D * D + 16 * D * D
+    for P in (262144, 2097152):
+        pts = torch.rand(P, 3, device="cuda", generator=g) * 2.01 - 1.005
+        ms = _time(lambda: vae.query(ctx, pts), iters=3, warm=1)
+        res[f"query_{P}"] = {"ms": ms, "tflops": flop_pt * P / ms / 1e9}
+    # the reference's recipe: fp32 modules under fp16 autocast, <= 10000 points per vae.decode call, trunk recomputed per call
+    sdc = {k: v.cuda() for k, v in sd.items()}
+    for P in (262144, 2097152):
+        pts = torch.rand(1, P, 3, device="cuda", generator=g) * 2.01 - 1.005
+
+        def recipe():
+            with torch.autocast("cuda", dtype=torch.float16):
+                for i in range(0, P, 10000):
+                    ref.decode_fp32(sdc, z[None], pts[:, i:i + 10000], 8, 16)
+
+        ms = _time(recipe, iters=1, warm=1)
+        res[f"reference_recipe_{P}"] = {"ms": ms, "calls": (P + 9999) // 10000}
+    t = {}
+
+    def extract():
+        grid = refine_octree(ref.sphere, ref.BOUNDS, 9)
+        torch.cuda.synchronize()
+        t["refine"] = time.time()
+        v, f = mesh_from_grid(grid, ref.BOUNDS, 9)
+        t["nv"], t["nf"] = len(v), len(f)
+        return grid
+
+    for _ in range(2):
+        torch.cuda.synchronize()
+        t0 = time.time()
+        grid = extract()
+        t1 = time.time()
+    res["sphere_depth9"] = {"refine_ms": (t["refine"] - t0) * 1e3, "dmc_ms": (t1 - t["refine"]) * 1e3,
+                            "total_ms": (t1 - t0) * 1e3, "vertices": t["nv"], "faces": t["nf"],
+                            "queried": int(torch.isfinite(grid).sum())}
+
+
 GROUPS = {
     "elementwise": group_elementwise, "gemm": group_gemm, "attn": group_attn, "attn_more": group_attn_more,
-    "gemm_perf": group_gemm_perf, "attn_perf": group_attn_perf,
+    "gemm_perf": group_gemm_perf, "attn_perf": group_attn_perf, "vae_decode": group_vae_decode,
 }
 TAG = os.environ.get("AMB_PROBE_TAG", "")
 if os.environ.get("AMB_PROBE_LIB"):  # bring-up only: probe an experimental build (tools/build_variant.sh) instead of the product library
