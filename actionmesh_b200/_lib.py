@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libactionmesh_b200.so")
 
-ABI_VERSION = 15
+ABI_VERSION = 16
 
 EXPORTS = [
     "amb_last_error", "amb_abi_version", "amb_device_info", "amb_cfg_euler_step", "amb_layernorm",
@@ -18,7 +18,7 @@ EXPORTS = [
     "amb_displacement_out", "amb_split3_bf16", "amb_softmax_split3", "amb_resize_h_u8", "amb_resize_v_normalize", "amb_alpha_stats", "amb_composite_crop_pad", "amb_nearest_neighbors", "amb_add_bias_rows", "amb_gemm_bf16", "amb_flash_attn_fwd", "amb_attn_small_f32",
     "amb_scan_scratch_ints", "amb_octree_near_surface", "amb_octree_dilate", "amb_octree_mark_upsampled",
     "amb_octree_count_points", "amb_octree_emit_points", "amb_grid_fill", "amb_grid_replace", "amb_grid_scatter",
-    "amb_dmc_count", "amb_dmc_emit",
+    "amb_dmc_count", "amb_dmc_emit", "amb_farthest_point_sample", "amb_gaussian_sample",
 ]
 
 
@@ -121,6 +121,10 @@ def load_library() -> C.CDLL:
     lib.amb_dmc_count.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.amb_dmc_emit.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]
+    lib.amb_farthest_point_sample.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_int,
+                                              C.c_void_p, C.c_void_p]
+    lib.amb_gaussian_sample.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if name != "amb_last_error":

@@ -575,3 +575,61 @@ def dual_marching_cubes(grid: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]
                                 verts.data_ptr(), faces.data_ptr(), _stream()), "amb_dmc_emit")
     launch_count += 9
     return verts[:nv], faces[:nf]
+
+
+# ---- mesh input: the TripoSG VAE encoder's point sampling and posterior (csrc/point_sampling.cu) ---------------------------
+FPS_MAX_POINTS = 16384
+
+
+def farthest_point_sample(points_xyz_view: torch.Tensor, k: int, start) -> torch.Tensor:
+    """Farthest-point sampling of (B, N, >=3) fp32 points (any row and batch stride: the xyz of (B, N, 6) surface rows are
+    read in place) -> (B, k) int64 indices, the first of each row `start[b]`; ties go to the lowest index.  `start`: (B,)
+    int64 on the host (range-checked) or on the device (caller's guarantee).  N <= 16384."""
+    global launch_count
+    _need(points_xyz_view, torch.float32, "points")
+    p = points_xyz_view
+    assert p.dim() == 3 and p.shape[2] >= 3 and p.stride(2) == 1
+    B, N = p.shape[0], p.shape[1]
+    start = torch.as_tensor(start, dtype=torch.int64).reshape(-1)
+    if start.numel() != B:
+        raise _lib.AmbError(f"farthest_point_sample: {start.numel()} start indices for a batch of {B}")
+    if not start.is_cuda:
+        if B and (int(start.min()) < 0 or int(start.max()) >= N):
+            raise _lib.AmbError(f"farthest_point_sample: start index outside [0, {N})")
+        start = start.to(p.device)
+    _need(start, torch.int64, "start")
+    out = torch.empty(B, int(k), dtype=torch.int64, device=p.device)
+    with _Timed("fps", (B, N, int(k))):
+        rc = _lib.load_library().amb_farthest_point_sample(p.data_ptr(), B, N, p.stride(1), p.stride(0) if B > 1 else N * p.stride(1),
+                                                           start.contiguous().data_ptr(), int(k), out.data_ptr(), _stream())
+    _lib.check(rc, "amb_farthest_point_sample")
+    launch_count += 1
+    return out
+
+
+def gaussian_sample(params: torch.Tensor, eps: Optional[torch.Tensor] = None, *, z: Optional[torch.Tensor] = None,
+                    logvar: Optional[torch.Tensor] = None, std: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+    """DiagonalGaussianDistribution on fp32 `params` (rows, >= 2C) (any row stride; C from the outputs' width):
+    logvar = clamp(params[:, C:2C], -30, 20), std = exp(0.5 logvar), z = params[:, :C] + std * eps.  Writes whichever of
+    z / logvar / std is given (contiguous (rows, C) fp32); with `eps` and no `z`, allocates and returns z."""
+    global launch_count
+    _need(params, torch.float32, "params")
+    assert params.dim() == 2 and params.stride(1) == 1
+    rows = params.shape[0]
+    if eps is not None and z is None:
+        z = torch.empty(eps.shape, dtype=torch.float32, device=params.device)
+    outs = [t for t in (z, logvar, std) if t is not None]
+    if not outs:
+        raise _lib.AmbError("gaussian_sample: nothing to write")
+    C_ = outs[0].shape[-1]
+    for t, nme in ((z, "z"), (logvar, "logvar"), (std, "std"), (eps, "eps")):
+        if t is not None:
+            _need(t, torch.float32, nme)
+            assert t.is_contiguous() and t.numel() == rows * C_, f"{nme}: expected {rows} x {C_} contiguous values"
+    if params.shape[1] < 2 * C_:
+        raise _lib.AmbError(f"gaussian_sample: params have {params.shape[1]} columns, need {2 * C_}")
+    rc = _lib.load_library().amb_gaussian_sample(params.data_ptr(), params.stride(0), rows, C_, _ptr(eps), _ptr(z), _ptr(logvar),
+                                                 _ptr(std), _stream())
+    _lib.check(rc, "amb_gaussian_sample")
+    launch_count += 1
+    return z

@@ -20,6 +20,7 @@ import os
 from dataclasses import dataclass
 from typing import Callable, List, Optional
 
+import numpy as np
 import torch
 
 from ._lib import AmbError
@@ -372,6 +373,13 @@ class ActionMeshB200Pipeline:
             input.frames = self.image_process.process_images(input.frames)
 
         latent_bank, anchor_mesh = self.init_banks_from_anchor(input, seed)          # Stage 0
+        ordered = self._animate(input, latent_bank, anchor_mesh.vertices, anchor_mesh.faces, anchor_mesh.vertex_normals, seed)
+        f_np = torch.as_tensor(anchor_mesh.faces).to(torch.int64).numpy()
+        return [_make_output_mesh(v.cpu().numpy(), f_np) for v in ordered]
+
+    def _animate(self, input, latent_bank: LatentBank, vertices, faces, vertex_normals, seed: int) -> list:
+        """DinoV2 on all frames, Stage I from the seeded `latent_bank`, then Stage II from the anchor mesh -> the (V, 3)
+        vertex tensors of every output timestep, in order."""
         self._load_image_encoder()
         vin = VideoInput(list(input.frames), input.timesteps)
         self._load_temporal_denoiser()
@@ -382,23 +390,116 @@ class ActionMeshB200Pipeline:
         latent_bank = stages.generate_3d_latents(vin, context, latent_bank, seed=seed)   # Stage I
         self._unload_model("temporal_3D_denoiser")
         dev = self._target_device
-        verts = torch.as_tensor(anchor_mesh.vertices, dtype=torch.float32).to(dev)
-        faces = torch.as_tensor(anchor_mesh.faces).to(torch.int64)
-        normals = torch.as_tensor(anchor_mesh.vertex_normals, dtype=torch.float32).to(dev)
+        verts = torch.as_tensor(vertices, dtype=torch.float32).to(dev)
+        faces = torch.as_tensor(faces).to(torch.int64)
+        normals = torch.as_tensor(vertex_normals, dtype=torch.float32).to(dev)
         stages._faces_holder["faces"] = faces
         vb = VertexBank(faces=faces)
         vb.update(timesteps=input.timesteps[[self.cfg.anchor_idx]], vertices=[verts])
         vb = stages.generate_mesh_animation(latent_bank, vb, normals)               # Stage II
         self._unload_model("temporal_3D_vae")
         ordered, _ = vb.get_ordered()
-        out = []
-        f_np = faces.cpu().numpy()
-        try:
-            import trimesh
+        return ordered
 
-            for v in ordered:
-                out.append(trimesh.Trimesh(vertices=v.cpu().numpy(), faces=f_np, process=False))
+
+def _make_output_mesh(vertices, faces):
+    """trimesh.Trimesh(vertices, faces, process=False) as the reference returns, or the package's `Mesh`."""
+    try:
+        import trimesh
+
+        return trimesh.Trimesh(vertices=vertices, faces=faces, process=False)
+    except ImportError:
+        return Mesh(vertices=vertices, faces=faces)
+
+
+class ActionMeshB200PipelineWithMeshInput(ActionMeshB200Pipeline):
+    """{video + 3D mesh} -> 4D: `ActionMeshPipelineWithMeshInput` (reference actionmesh/pipeline_with_3d.py:27-240) on the
+    CUDA path.  The user's mesh is merged and cleaned, normalized, sampled (16384 surface points with face normals) and
+    encoded by the TripoSG VAE encoder (`B200TripoSGVAE.encode_to_latent`) into the anchor latent; Stage I and Stage II are
+    the base pipeline's.  The outputs are denormalized and expanded back to the input's own vertices and faces
+    (`pre_merge_faces`), so its UVs and textures still apply.  No mesh post-processing runs on this path, as in the reference.
+
+    The VAE is `B200TripoSGVAE.from_pretrained(f"{triposg_weights_dir}/vae")`, or assigned directly (`pipe.vae = model`).
+    Unlike the reference, which passes no seed to the encoder's point sampling and posterior sample, both are seeded from
+    `seed`, so two calls with the same seed give the same meshes.  Like the reference, `anchor_mesh` is modified in place."""
+
+    def __init__(self, *args, triposg_weights_dir: str = "pretrained_weights/TripoSG", **kwargs):
+        super().__init__(*args, **kwargs)
+        self._triposg_weights_dir = triposg_weights_dir
+        self.vae = None
+
+    def _load_vae(self) -> None:
+        if self.vae is None:
+            from .triposg_vae import B200TripoSGVAE
+
+            self.vae = B200TripoSGVAE.from_pretrained(os.path.join(self._triposg_weights_dir, "vae"), device=self._target_device)
+        self.vae.to(self._target_device)
+
+    def to(self, device) -> "ActionMeshB200PipelineWithMeshInput":
+        super().to(device)
+        if not self._lazy_loading:
+            self._load_vae()
+        return self
+
+    def init_banks_from_anchor(self, input, anchor_mesh, seed: int = 44):
+        """pipeline_with_3d.py:60-125 -> (latent_bank, vertex_bank, normalization, vertex_merge_map, pre_merge_faces).
+        `vertex_bank` holds the merged, normalized anchor vertices at the anchor timestep (its `faces` the merged faces):
+        the vertex-only counterpart of the reference's MeshBank."""
+        from .mesh_input import merge_and_clean_mesh, normalize_mesh, sample_surface
+
+        vertex_merge_map, pre_merge_faces = merge_and_clean_mesh(anchor_mesh)
+        anchor_mesh, params = normalize_mesh(anchor_mesh)
+        surface = sample_surface(anchor_mesh, n_points=16384, seed=seed, with_normals=True, device=self._target_device,
+                                 dtype=torch.float32)
+        anchor_latent = self.vae.encode_to_latent(surface, seed=seed, generator=torch.Generator().manual_seed(seed))
+        anchor_t = input.timesteps[[self.cfg.anchor_idx]]
+        latent_bank = LatentBank(empty_dims=self._denoiser_latent_shape)
+        latent_bank.update(timesteps=anchor_t, latents=anchor_latent.to(dtype=torch.float32))
+        faces = torch.as_tensor(anchor_mesh.faces).to(torch.int64)
+        vertex_bank = VertexBank(faces=faces)
+        vertex_bank.update(timesteps=anchor_t, vertices=[torch.as_tensor(anchor_mesh.vertices, dtype=torch.float32)])
+        return latent_bank, vertex_bank, params, vertex_merge_map, pre_merge_faces
+
+    @torch.no_grad()
+    def __call__(self, input, anchor_mesh, seed: int = 44, stage_0_steps: Optional[int] = None,
+                 face_decimation: Optional[int] = None, floaters_threshold: Optional[float] = None,
+                 stage_1_steps: Optional[int] = None, guidance_scales: Optional[List[float]] = None,
+                 anchor_idx: Optional[int] = None) -> list:
+        """{video + 3D mesh} -> 4D (pipeline_with_3d.py:127-240): the animated meshes with the input mesh's own vertices
+        and faces, ordered by timestep."""
+        from .mesh_input import denormalize_mesh
+
+        if stage_0_steps is not None:
+            self.cfg.model.image_to_3D_denoiser.num_inference_steps = stage_0_steps
+        if stage_1_steps is not None:
+            self.scheduler.num_inference_steps = stage_1_steps
+        if guidance_scales is not None:
+            self.cf_guidance.guidance_scales = guidance_scales
+        if face_decimation is not None:
+            self.mesh_process.face_decimation = face_decimation
+        if floaters_threshold is not None:
+            self.mesh_process.floaters_threshold = floaters_threshold
+        if anchor_idx is not None:
+            self.cfg.anchor_idx = anchor_idx
+        if self.background_removal is not None:
+            input.frames = self.background_removal.process_images(input.frames)
+        if self.image_process is not None:
+            input.frames = self.image_process.process_images(input.frames)
+
+        self._load_vae()
+        latent_bank, vertex_bank, params, vertex_merge_map, pre_merge_faces = self.init_banks_from_anchor(input, anchor_mesh, seed)
+        self._unload_model("vae")
+        verts = vertex_bank.get(timesteps=input.timesteps[[self.cfg.anchor_idx]])[0]
+        faces = vertex_bank.faces
+        try:
+            import trimesh  # the reference's source of vertex normals (mesh_processor.py:98)
+
+            normals = trimesh.Trimesh(vertices=verts.numpy(), faces=faces.numpy(), process=False).vertex_normals.copy()
         except ImportError:
-            for v in ordered:
-                out.append(Mesh(vertices=v.cpu().numpy(), faces=f_np))
+            normals = _vertex_normals(verts, faces)
+        ordered = self._animate(input, latent_bank, verts, faces, normals, seed)
+        out = []
+        for v in ordered:
+            m = denormalize_mesh(Mesh(vertices=v.cpu().numpy().astype(np.float64), faces=None), params)
+            out.append(_make_output_mesh(np.asarray(m.vertices)[vertex_merge_map], pre_merge_faces))
         return out

@@ -10,6 +10,12 @@ latent (`prepare`); the reference recomputes them in every `vae.decode` call.  P
 fp32 accumulation, fp32 residual stream, LayerNorm statistics, coordinates and point embedding — the recipe and tolerance of
 Stage 0's DiT.  (The reference runs this model in fp16, pipeline.py:140-142; the fp32 modules are the yardstick.)
 There is no torch arithmetic on the path: torch allocates buffers and views them.
+
+The encoder side (`encode`, `encode_to_latent`) turns the surface samples of a user-supplied mesh into the anchor latent of
+the {video + 3D mesh} -> 4D pipeline: farthest-point sampling on the GPU (csrc/point_sampling.cu), then TripoSGEncoder (one
+cross-attention block from the sampled points to all surface points, then self-attention blocks) and `quant` on the same
+kernels, and the posterior sample in one elementwise kernel.  Coordinates, point embedding and FPS stay fp32; the reference
+rounds the surface to fp16 before embedding it (pipeline_with_3d.py:97-105) and runs the VAE in fp16.
 """
 from __future__ import annotations
 
@@ -33,7 +39,7 @@ INVALID = -10000.0                                                 # flash_extra
 
 @dataclass
 class TripoSGVAEConfig:
-    """Constructor arguments of TripoSGVAEModel (autoencoder_kl_triposg.py:221-233); the encoder's are accepted and unused."""
+    """Constructor arguments of TripoSGVAEModel (autoencoder_kl_triposg.py:221-233)."""
     in_channels: int = 3
     latent_channels: int = 64
     num_attention_heads: int = 8
@@ -53,6 +59,23 @@ class TripoSGVAEConfig:
     def query_dim(self) -> int:
         return self.in_channels * (2 * self.embed_frequency + 1)
 
+    @property
+    def encoder_head_dim(self) -> int:
+        return self.width_encoder // self.num_attention_heads
+
+    @property
+    def encoder_in_dim(self) -> int:
+        """[embed(xyz) | normal]: the encoder's proj_in input (autoencoder_kl_triposg.py:250-252,442-451)."""
+        return self.query_dim + self.in_channels
+
+    def encoder_supported(self) -> Optional[str]:
+        """None when the encoder side runs on this build, else the reason it does not."""
+        if self.encoder_head_dim not in (64, 128) or self.encoder_head_dim * self.num_attention_heads != self.width_encoder:
+            return f"the encoder needs head_dim 64 or 128 (got width_encoder {self.width_encoder} / {self.num_attention_heads} heads)"
+        if self.width_encoder not in (256, 512, 1024, 2048, 4096):
+            return f"unsupported width_encoder {self.width_encoder}"
+        return None
+
 
 @dataclass
 class AnchorMesh(Mesh):
@@ -66,6 +89,42 @@ class LatentContext:
     kv: torch.Tensor
     k: torch.Tensor
     v: torch.Tensor
+
+
+class DiagonalGaussianDistribution:
+    """The posterior of vae.py:8-36 over fp32 `parameters` (..., 2C) = [mean | logvar] (the `quant` output, read in place):
+    `mean` is a view, `logvar` (clamped to [-30, 20]) and `std` = exp(0.5 logvar) come from one kernel, and
+    `sample(generator)` = mean + std * eps with eps ~ torch.randn from `generator` (on the generator's device)."""
+
+    def __init__(self, parameters: torch.Tensor):
+        C = parameters.shape[-1] // 2
+        self.parameters = parameters
+        self._rows = parameters.reshape(-1, 2 * C)
+        self.mean = parameters[..., :C]
+        self.logvar = torch.empty(self.mean.shape, dtype=torch.float32, device=parameters.device)
+        self.std = torch.empty_like(self.logvar)
+        ops.gaussian_sample(self._rows, logvar=self.logvar.view(-1, C), std=self.std.view(-1, C))
+
+    @torch.no_grad()
+    def sample(self, generator: Optional[torch.Generator] = None, eps: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """mean + std * eps; `eps` (same shape as mean) replaces the draw when given."""
+        dev = self.parameters.device
+        if eps is None:
+            gdev = generator.device if generator is not None else dev
+            eps = torch.randn(self.mean.shape, generator=generator, device=gdev, dtype=torch.float32)
+        eps = eps.to(device=dev, dtype=torch.float32).contiguous()
+        z = torch.empty(self.mean.shape, dtype=torch.float32, device=dev)
+        ops.gaussian_sample(self._rows, eps.view(-1, self.mean.shape[-1]), z=z.view(-1, self.mean.shape[-1]))
+        return z
+
+    def mode(self) -> torch.Tensor:
+        return self.mean
+
+
+@dataclass
+class EncoderOutput:
+    """diffusers' AutoencoderKLOutput: the posterior of `B200TripoSGVAE.encode`."""
+    latent_dist: DiagonalGaussianDistribution
 
 
 def octree_resolutions(octree_depth: int, min_resolution: int = 63, mini_grid_num: int = 4) -> list[int]:
@@ -142,8 +201,9 @@ def make_mesh(vertices: np.ndarray, faces: np.ndarray):
 
 
 class B200TripoSGVAE:
-    """Decoder side of TripoSGVAEModel: same constructor arguments, state-dict keys (`post_quant.*`, `decoder.*`; the
-    encoder's keys are ignored), `from_pretrained(f"{triposg_dir}/vae")` and `decode(z, sampled_points)`."""
+    """TripoSGVAEModel on the CUDA path: same constructor arguments, state-dict keys (`post_quant.*`, `decoder.*`, and the
+    encoder side's `encoder.*`, `quant.*` when present), `from_pretrained(f"{triposg_dir}/vae")`, `decode(z, sampled_points)`
+    and, for a user-supplied mesh, `encode(surface)` / `encode_to_latent(surface)` (actionmesh/external/triposg.py:103-172)."""
 
     QUERY_CHUNK = 262144   # query rows per pass: ~4.6 GB of activations at width 1024
 
@@ -161,7 +221,9 @@ class B200TripoSGVAE:
         self._device = torch.device("cpu")
         self._w: dict = {}
         self._loaded = False
+        self._has_encoder = False
         self._qpad = 64 * ((c.query_dim + 63) // 64)
+        self._epad = 64 * ((c.encoder_in_dim + 63) // 64)
 
     # ------------------------------------------------------------------ nn.Module-like surface
     @property
@@ -202,7 +264,8 @@ class B200TripoSGVAE:
     @ops.on_device
     def load_state_dict(self, sd: dict) -> None:
         """Pack the weights: bf16 GEMM operands (self-attention QKV fused with the head split folded in, cross K/V likewise,
-        proj_query K-padded to 64, proj_out N-padded to 64 and negated); biases and norm weights fp32."""
+        proj_query K-padded to 64, proj_out N-padded to 64 and negated); biases and norm weights fp32.  The encoder side
+        (`encoder.*`, `quant.*`: proj_in K-padded 54 -> 64) is packed too when the dict has it."""
         c = self.config
         dev = self._device
         if dev.type != "cuda":
@@ -215,14 +278,13 @@ class B200TripoSGVAE:
         def W(name):
             return f32(name).to(torch.bfloat16).contiguous()
 
-        w = {"post_quant.w": W("post_quant.weight"), "post_quant.b": f32("post_quant.bias")}
-        for i in range(L + 1):
-            p, q = f"decoder.blocks.{i}.", f"b{i}."
-            norm_attn, attn = ("norm2", "attn2") if i == L else ("norm1", "attn1")
+        def block(p, q, cross):
+            """DiTBlock `p` (self- or cross-attention, no qk-norm, no qkv bias) -> packed entries under prefix `q`."""
+            norm_attn, attn = ("norm2", "attn2") if cross else ("norm1", "attn1")
             for src, dst in ((norm_attn, "norm_attn"), ("norm3", "norm_ff")):
                 w[q + dst + ".g"], w[q + dst + ".b"] = f32(p + src + ".weight"), f32(p + src + ".bias")
             wq, wk, wv = (f32(p + f"{attn}.to_{n}.weight") for n in "qkv")
-            if i < L:
+            if not cross:
                 w[q + "qkv"] = repack_self_qkv(wq, wk, wv, H).to(torch.bfloat16).contiguous()
             else:
                 w[q + "q"] = wq.to(torch.bfloat16).contiguous()
@@ -231,6 +293,10 @@ class B200TripoSGVAE:
             w[q + "o.w"], w[q + "o.b"] = W(p + f"{attn}.to_out.0.weight"), f32(p + f"{attn}.to_out.0.bias")
             w[q + "ff1.w"], w[q + "ff1.b"] = W(p + "ff.net.0.proj.weight"), f32(p + "ff.net.0.proj.bias")
             w[q + "ff2.w"], w[q + "ff2.b"] = W(p + "ff.net.2.weight"), f32(p + "ff.net.2.bias")
+
+        w = {"post_quant.w": W("post_quant.weight"), "post_quant.b": f32("post_quant.bias")}
+        for i in range(L + 1):
+            block(f"decoder.blocks.{i}.", f"b{i}.", cross=i == L)
         pq = torch.zeros(D, self._qpad, dtype=torch.float32, device=dev)
         pq[:, :c.query_dim].copy_(f32("decoder.proj_query.weight"))
         w["proj_query.w"], w["proj_query.b"] = pq.to(torch.bfloat16), f32("decoder.proj_query.bias")
@@ -241,6 +307,19 @@ class B200TripoSGVAE:
         pb = torch.zeros(64, dtype=torch.float32, device=dev)
         pb[:1].copy_(f32("decoder.proj_out.bias"))
         w["proj_out.w"], w["proj_out.b"] = po.neg().to(torch.bfloat16), pb.neg()
+        self._has_encoder = "quant.weight" in sd
+        if self._has_encoder:
+            why = c.encoder_supported()
+            if why is not None:
+                raise AmbError(f"B200TripoSGVAE: {why}")
+            # block 0 cross-attends from the sampled points to all surface points; blocks 1..L are self-attention
+            for i in range(c.num_layers_encoder + 1):
+                block(f"encoder.blocks.{i}.", f"e{i}.", cross=i == 0)
+            pi = torch.zeros(c.width_encoder, self._epad, dtype=torch.float32, device=dev)
+            pi[:, :c.encoder_in_dim].copy_(f32("encoder.proj_in.weight"))
+            w["proj_in.w"], w["proj_in.b"] = pi.to(torch.bfloat16), f32("encoder.proj_in.bias")
+            w["enc_norm_out.g"], w["enc_norm_out.b"] = f32("encoder.norm_out.weight"), f32("encoder.norm_out.bias")
+            w["quant.w"], w["quant.b"] = W("quant.weight"), f32("quant.bias")
         self._w = w
         self._loaded = True
 
@@ -259,8 +338,9 @@ class B200TripoSGVAE:
             if bias:
                 sd[name + ".bias"] = (torch.rand(out_f, generator=g, device=dev) * 2 - 1) * bound * scale
 
-        def ln(name):
-            sd[name + ".weight"], sd[name + ".bias"] = torch.ones(D, device=dev), torch.zeros(D, device=dev)
+        def ln(name, width=None):
+            width = width or D
+            sd[name + ".weight"], sd[name + ".bias"] = torch.ones(width, device=dev), torch.zeros(width, device=dev)
 
         sd = {}
         lin("post_quant", D, c.latent_channels)
@@ -279,6 +359,26 @@ class B200TripoSGVAE:
             lin(p + f"{a}.to_out.0", D, D, scale=rs)
             lin(p + "ff.net.0.proj", 4 * D, D)
             lin(p + "ff.net.2", D, 4 * D, scale=rs)
+        if c.encoder_supported() is None:
+            # encoder from its own generator, so the decoder's weights are the same with or without it
+            g = torch.Generator(device=dev).manual_seed(seed + 1)
+            We, Le = c.width_encoder, c.num_layers_encoder
+            rs = 1.0 / math.sqrt(Le + 1)
+            lin("encoder.proj_in", We, c.encoder_in_dim)
+            lin("quant", 2 * c.latent_channels, We)
+            ln("encoder.norm_out", We)
+            for i in range(Le + 1):
+                p = f"encoder.blocks.{i}."
+                a = "attn2" if i == 0 else "attn1"
+                ln(p + ("norm2" if i == 0 else "norm1"), We)
+                ln(p + "norm3", We)
+                if i == 0:
+                    ln(p + "attn2.norm_cross", We)
+                for n in ("to_q", "to_k", "to_v"):
+                    lin(p + f"{a}.{n}", We, We, bias=False)
+                lin(p + f"{a}.to_out.0", We, We, scale=rs)
+                lin(p + "ff.net.0.proj", 4 * We, We)
+                lin(p + "ff.net.2", We, 4 * We, scale=rs)
         self.load_state_dict(sd)
 
     # ------------------------------------------------------------------ decode
@@ -358,6 +458,99 @@ class B200TripoSGVAE:
             logits = self.query(self.prepare(z[b]), sampled_points[b].reshape(P, 3))
             out[b, :, 0].copy_(logits[:, 0])
         return out if return_dict else (out,)
+
+    # ------------------------------------------------------------------ encode
+    @ops.on_device
+    @torch.no_grad()
+    def encode_points(self, x_kv: torch.Tensor, x_q: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """TripoSGEncoder + quant for one shape (autoencoder_kl_triposg.py:26-87,439-457): all surface points x_kv (N, 6) and
+        the sampled points x_q (T, 6), fp32 [xyz | normal] rows -> (T, 2 * latent_channels) fp32 `quant` output."""
+        if not self._loaded or not self._has_encoder:
+            raise AmbError("B200TripoSGVAE: encoder weights not loaded")
+        c, w, dev = self.config, self._w, self._device
+        N, T = x_kv.shape[0], x_q.shape[0]
+        D, H, dh, L = c.width_encoder, c.num_attention_heads, c.encoder_head_dim, c.num_layers_encoder
+        bf, f32 = torch.bfloat16, torch.float32
+        E = lambda *s, dtype=bf: torch.empty(*s, dtype=dtype, device=dev)
+        if out is None:
+            out = E(T, 2 * c.latent_channels, dtype=f32)
+        h, xn, qkv, att, ff = E(T, D, dtype=f32), E(T, D), E(T, 3 * D), E(T, D), E(T, 4 * D)
+        ctx, ctxn = E(N, D, dtype=f32), E(N, D)
+        F, pi = c.embed_frequency, c.embed_include_pi
+        # x_kv = [embed(xyz) | normal] of every surface point, x_q the same of the sampled points; one shared proj_in
+        ekv = ops.cast_bf16(ops.point_embedding(x_kv.detach().to(device=dev, dtype=f32).contiguous(), F, pi, self._epad))
+        eq = ops.cast_bf16(ops.point_embedding(x_q.detach().to(device=dev, dtype=f32).contiguous(), F, pi, self._epad))
+        ops.gemm(eq, w["proj_in.w"], h, bias=w["proj_in.b"], tag="vae_encoder")
+        ops.gemm(ekv, w["proj_in.w"], ctx, bias=w["proj_in.b"], tag="vae_encoder")
+        del ekv, eq
+        scale = 1.0 / math.sqrt(dh)
+        # block 0: cross-attention to the norm_cross'ed surface tokens
+        q = "e0."
+        ops.layernorm(ctx, w[q + "norm_cross.g"], w[q + "norm_cross.b"], 1e-5, out=ctxn)
+        kv = ops.gemm(ctxn, w[q + "kv"], E(N, 2 * D), tag="vae_encoder")          # [K(h,d) | V(h,d)]
+        del ctx, ctxn
+        ops.layernorm(h, w[q + "norm_attn.g"], w[q + "norm_attn.b"], 1e-5, out=xn)
+        qb = ops.gemm(xn, w[q + "q"], E(T, D), tag="vae_encoder")
+        ops.flash_attn(qb.view(1, T, H, dh), kv[:, :D].view(1, N, H, dh), kv[:, D:].view(1, N, H, dh), att.view(1, T, H, dh),
+                       scale, tag="vae_encoder_attn")
+        del qb, kv
+        for i in range(L + 1):
+            q = f"e{i}."
+            if i > 0:
+                ops.layernorm(h, w[q + "norm_attn.g"], w[q + "norm_attn.b"], 1e-5, out=xn)
+                ops.gemm(xn, w[q + "qkv"], qkv, tag="vae_encoder")
+                ops.flash_attn(qkv[:, 0:D].view(1, T, H, dh), qkv[:, D:2 * D].view(1, T, H, dh),
+                               qkv[:, 2 * D:].view(1, T, H, dh), att.view(1, T, H, dh), scale, tag="vae_encoder_attn")
+            ops.gemm(att, w[q + "o.w"], h, bias=w[q + "o.b"], residual=h, tag="vae_encoder")
+            ops.layernorm(h, w[q + "norm_ff.g"], w[q + "norm_ff.b"], 1e-5, out=xn)
+            ops.gemm(xn, w[q + "ff1.w"], ff, bias=w[q + "ff1.b"], act=1, tag="vae_encoder")
+            ops.gemm(ff, w[q + "ff2.w"], h, bias=w[q + "ff2.b"], residual=h, tag="vae_encoder")
+        ops.layernorm(h, w["enc_norm_out.g"], w["enc_norm_out.b"], 1e-5, out=xn)
+        ops.gemm(xn, w["quant.w"], out, bias=w["quant.b"], tag="vae_encoder")
+        return out
+
+    @ops.on_device
+    @torch.no_grad()
+    def sample_features(self, x: torch.Tensor, num_tokens: int = 2048, seed: Optional[int] = None,
+                        generator: Optional[torch.Generator] = None) -> tuple[torch.Tensor, torch.Tensor]:
+        """TripoSGVAE._sample_features (actionmesh/external/triposg.py:113-151): (B, N, 6) fp32 CUDA surface -> (the sampled
+        rows (B, num_tokens, 6), their indices into the 4 * num_tokens subset (B, num_tokens) int64).
+
+        The subset is `np.random.default_rng(seed).choice(N, 4 * num_tokens, replace=4 * num_tokens > N)` on the host, the
+        reference's exact call; farthest-point sampling then runs on the GPU from `torch.randint(high=4 * num_tokens,
+        size=(1,), generator=generator)` per batch element."""
+        B, N = x.shape[:2]
+        m = 4 * num_tokens
+        if m > ops.FPS_MAX_POINTS:
+            raise AmbError(f"num_tokens {num_tokens}: farthest-point sampling supports 4 * num_tokens <= {ops.FPS_MAX_POINTS}")
+        subset = np.random.default_rng(seed).choice(N, m, replace=m > N)
+        selected = x[:, torch.from_numpy(subset).to(x.device)]                       # (B, m, 6), a gather
+        gdev = generator.device if generator is not None else torch.device("cpu")
+        start = torch.cat([torch.randint(high=m, size=(1,), generator=generator, device=gdev) for _ in range(B)])
+        idx = ops.farthest_point_sample(selected, num_tokens, start)
+        return selected[torch.arange(B, device=x.device)[:, None], idx], idx
+
+    @torch.no_grad()
+    def encode(self, x: torch.Tensor, return_dict: bool = True, num_tokens: int = 2048, seed: Optional[int] = None,
+               generator: Optional[torch.Generator] = None):
+        """TripoSGVAEModel.encode with TripoSGVAE's sampling (autoencoder_kl_triposg.py:439-479, external/triposg.py:113-151):
+        (B, N, 6) surface [xyz | normal] -> `.latent_dist`, a `DiagonalGaussianDistribution` of (B, num_tokens, C).
+        `seed` fixes the host subset, `generator` the FPS start (and is the natural one to pass to `.sample`)."""
+        x = x.detach().to(device=self._device, dtype=torch.float32).contiguous()
+        with torch.cuda.device(self._device):
+            sampled, _ = self.sample_features(x, num_tokens, seed, generator)
+            params = torch.empty(x.shape[0], num_tokens, 2 * self.config.latent_channels, dtype=torch.float32, device=self._device)
+            for b in range(x.shape[0]):
+                self.encode_points(x[b], sampled[b], out=params[b])
+            posterior = DiagonalGaussianDistribution(params)
+        return EncoderOutput(latent_dist=posterior) if return_dict else (posterior,)
+
+    @torch.no_grad()
+    def encode_to_latent(self, surface: torch.Tensor, seed: Optional[int] = None,
+                         generator: Optional[torch.Generator] = None) -> torch.Tensor:
+        """TripoSGVAE.encode_to_latent (external/triposg.py:153-172): (B, N, 6) surface -> posterior sample (B, 2048, C) fp32.
+        With both `seed` and `generator` given the result is reproducible (the reference passes neither)."""
+        return self.encode(surface, seed=seed, generator=generator).latent_dist.sample(generator)
 
     # ------------------------------------------------------------------ mesh
     @torch.no_grad()

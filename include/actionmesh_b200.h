@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define AMB_ABI_VERSION 15
+#define AMB_ABI_VERSION 16
 
 typedef void* amb_stream_t; /* cudaStream_t */
 
@@ -242,6 +242,23 @@ int amb_dmc_count(const float* grid, int n, uint8_t* cases, int32_t* vertex_scra
                   amb_stream_t stream);
 int amb_dmc_emit(const float* grid, int n, const uint8_t* cases, const int32_t* vertex_scratch, const int32_t* face_scratch,
                  int32_t* vertex_offsets, float* vertices, int32_t* faces, amb_stream_t stream);
+
+/* ---- mesh input: the TripoSG VAE encoder's point sampling and posterior (csrc/point_sampling.cu) -------------------------
+ *  farthest_point_sample: replaces pytorch3d's sample_farthest_points(points[..., :3], K, random_start_point=True) called by
+ *    TripoSGVAE._sample_features (actionmesh/external/triposg.py:113-151, model/utils/pointcloud_sampling.py:54-62).
+ *    points: fp32, point i of batch element b has its x, y, z at points + b * batch_stride + i * ld (+0, +1, +2), so the xyz
+ *    of wider rows (xyz + normal) is read in place.  start: (batch) int64 DEVICE array in [0, n).  out: (batch, k) int64.
+ *    out[b, 0] = start[b]; every point keeps d = min over the selected points of ((dx*dx) + (dy*dy)) + (dz*dz), fp32 with each
+ *    operation rounded on its own, initialised to +inf; out[b, r] = argmax d with ties to the lowest index (once every d is
+ *    0 that is index 0 again, as a plain argmax).  Deterministic.  1 <= n <= 16384.
+ *  gaussian_sample: DiagonalGaussianDistribution (third_party/TripoSG/triposg/models/autoencoders/vae.py:8-36) on the fp32
+ *    `quant` output (rows, >= 2C) with row stride ld: logvar = clamp(params[:, C:2C], -30, 20), std = exp(0.5 logvar),
+ *    z = params[:, :C] + std * eps.  eps, z, logvar, std_out: contiguous (rows, C) fp32; any of z, logvar, std_out may be
+ *    NULL (eps only needed with z). */
+int amb_farthest_point_sample(const float* points, int batch, int n, int64_t ld, int64_t batch_stride, const int64_t* start,
+                              int k, int64_t* out, amb_stream_t stream);
+int amb_gaussian_sample(const float* params, int64_t ld, int64_t rows, int channels, const float* eps, float* z,
+                        float* logvar, float* std_out, amb_stream_t stream);
 
 #ifdef __cplusplus
 }

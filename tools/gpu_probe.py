@@ -406,9 +406,53 @@ def group_vae_decode(res):
                             "queried": int(torch.isfinite(grid).sum())}
 
 
+def group_vae_encode(res):
+    """TripoSG VAE encoder of the mesh-input path at full width (512, 8 heads x 64, 8 layers; 16384 surface points -> 2048
+    tokens): the FPS kernel (8192 -> 2048), the encoder launch program, the whole encode_to_latent, and the reference's recipe
+    (the fp32 restatement under fp16 autocast).  pytorch3d's FPS, which the reference uses, is not installed and not timed.
+    FLOPs: proj_in 2 (T + N) 64 W, cross q/o 4 T W^2, cross K/V 4 N W^2, FF 16 T W^2 per block, self QKV/o 8 T W^2,
+    attention 4 T N W (cross) and 4 T^2 W (self), quant 2 T W 128."""
+    import torch
+
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import triposg_vae_encoder_ref as ref
+    import triposg_vae_ref as dref
+    from actionmesh_b200 import ops
+    from actionmesh_b200.triposg_vae import B200TripoSGVAE
+
+    res["card"] = _card()
+    W, L, T, N = 512, 8, 2048, 16384
+    sd = dref.make_state_dict(1024, 8, 1, seed=1)
+    enc = ref.make_encoder_state_dict(W, 8, L, seed=2)
+    sd.update(enc)
+    vae = B200TripoSGVAE(num_layers_decoder=1).to("cuda")
+    vae.load_state_dict(sd)
+    surface = ref.sphere_surface(N, 3).cuda()
+    sub = surface[:, :4 * T].contiguous()
+    start = torch.tensor([17], device="cuda")
+    res["fps_8192_2048"] = {"ms": _time(lambda: ops.farthest_point_sample(sub, T, start), iters=20, warm=3)}
+    sampled, _ = vae.sample_features(surface, T, seed=0, generator=torch.Generator().manual_seed(0))
+    attn = 4 * T * N * W + L * 4 * T * T * W
+    flop = 2 * (T + N) * 64 * W + 4 * T * W * W + 4 * N * W * W + (L + 1) * 16 * T * W * W + L * 8 * T * W * W + attn \
+        + 2 * T * W * 128
+    ms = _time(lambda: vae.encode_points(surface[0], sampled[0]), iters=10, warm=2)
+    res["encoder_program"] = {"ms": ms, "tflops": flop / ms / 1e9, "gflop": flop / 1e9, "attn_gflop": attn / 1e9}
+    res["encode_to_latent"] = {"ms": _time(lambda: vae.encode_to_latent(surface, seed=0, generator=torch.Generator().manual_seed(0)),
+                                           iters=10, warm=2)}
+    sdc = {k: v.cuda() for k, v in enc.items()}
+
+    def recipe():
+        with torch.autocast("cuda", dtype=torch.float16):
+            ref.encode_fp32(sdc, surface, sampled, 8, L)
+
+    ms = _time(recipe, iters=5, warm=2)
+    res["reference_recipe_encoder"] = {"ms": ms, "tflops": flop / ms / 1e9}
+
+
 GROUPS = {
     "elementwise": group_elementwise, "gemm": group_gemm, "attn": group_attn, "attn_more": group_attn_more,
     "gemm_perf": group_gemm_perf, "attn_perf": group_attn_perf, "vae_decode": group_vae_decode,
+    "vae_encode": group_vae_encode,
 }
 TAG = os.environ.get("AMB_PROBE_TAG", "")
 if os.environ.get("AMB_PROBE_LIB"):  # bring-up only: probe an experimental build (tools/build_variant.sh) instead of the product library
