@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libactionmesh_b200.so")
 
-ABI_VERSION = 16
+ABI_VERSION = 17
 
 EXPORTS = [
     "amb_last_error", "amb_abi_version", "amb_device_info", "amb_cfg_euler_step", "amb_layernorm",
@@ -19,6 +19,8 @@ EXPORTS = [
     "amb_scan_scratch_ints", "amb_octree_near_surface", "amb_octree_dilate", "amb_octree_mark_upsampled",
     "amb_octree_count_points", "amb_octree_emit_points", "amb_grid_fill", "amb_grid_replace", "amb_grid_scatter",
     "amb_dmc_count", "amb_dmc_emit", "amb_farthest_point_sample", "amb_gaussian_sample",
+    "amb_mesh_adjacency", "amb_mesh_edges", "amb_mesh_quadrics", "amb_mesh_collapse_select", "amb_mesh_collapse_apply",
+    "amb_mesh_compact_faces", "amb_mesh_compact_vertices", "amb_mesh_components", "amb_mesh_component_sizes",
 ]
 
 
@@ -125,6 +127,16 @@ def load_library() -> C.CDLL:
                                               C.c_void_p, C.c_void_p]
     lib.amb_gaussian_sample.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p]
+    P, I64 = C.c_void_p, C.c_int64
+    lib.amb_mesh_adjacency.argtypes = [P, I64, I64, P, P, P, P, P, P]
+    lib.amb_mesh_edges.argtypes = [P, I64, I64, P, P, P, P, P, P, P, P]
+    lib.amb_mesh_quadrics.argtypes = [P, P, I64, P, P, P, P, P]
+    lib.amb_mesh_collapse_select.argtypes = [P, P, P, I64, P, P, P, P, I64, P, P, P, P, P, P, P, P]
+    lib.amb_mesh_collapse_apply.argtypes = [P, I64, I64, P, P, P, C.c_uint64, P, P, P, P]
+    lib.amb_mesh_compact_faces.argtypes = [P, I64, P, P, P, C.c_int, P, P, P]
+    lib.amb_mesh_compact_vertices.argtypes = [P, I64, P, I64, P, P, P, P, P]
+    lib.amb_mesh_components.argtypes = [P, I64, I64, C.c_int, P, P, P]
+    lib.amb_mesh_component_sizes.argtypes = [P, I64, P, P]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if name != "amb_last_error":

@@ -2,6 +2,7 @@
 
 Same signatures and return values as the reference's actionmesh/preprocessing/mesh_processor.py:
   merge_and_clean_mesh   :37-82   merge seam duplicates, drop degenerate / duplicate faces and unreferenced vertices
+                                  (the rules are `clean_topology`, which B200MeshPostprocessor shares)
   normalize_mesh         :177-212 centre the bounding box, scale by 2 / max extent
   denormalize_mesh       :215-237 the inverse
   sample_surface         :245-285 area-weighted surface samples with their face normals -> (1, n, 3|6) tensor
@@ -25,21 +26,14 @@ def _arrays(mesh) -> tuple[np.ndarray, np.ndarray]:
     return np.asarray(mesh.vertices, dtype=np.float64), np.asarray(mesh.faces, dtype=np.int64).reshape(-1, 3)
 
 
-def merge_and_clean_mesh(mesh) -> tuple[np.ndarray, np.ndarray]:
-    """Merge duplicate vertices and clean the topology of `mesh` in place; -> (vertex_merge_map, pre_merge_faces).
-
-    Rules, in order:
+def clean_topology(verts: np.ndarray, faces: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
+    """The reference's topology clean-up (trimesh merge_vertices, remove_degenerate_faces, remove_duplicate_faces,
+    remove_unreferenced_vertices) on (V, 3) float64 vertices and (F, 3) int64 faces -> new (vertices, faces).  Rules, in order:
       1. vertices whose coordinates are equal after rounding to 8 decimals become one vertex, placed at the first of them;
          the merged vertices keep the order of their first occurrence;
       2. faces that use a vertex twice are dropped;
       3. faces that repeat an earlier face as a sorted index triple are dropped (the first one is kept);
-      4. vertices no face references are dropped.
-    vertex_merge_map (N_original,): for each original vertex, the index of the nearest merged vertex (cKDTree); as in the
-    reference every distance must be below 1e-6.  pre_merge_faces: a copy of the original (F_original, 3) faces."""
-    verts, faces = _arrays(mesh)
-    pre_merge_verts = verts.copy()
-    pre_merge_faces = np.array(mesh.faces, copy=True)
-
+      4. vertices no face references are dropped."""
     _, first, inverse = np.unique(np.round(verts, MERGE_DECIMALS) + 0.0, axis=0, return_index=True, return_inverse=True)
     order = np.argsort(first, kind="stable")           # merged vertices in order of first occurrence
     rank = np.empty_like(order)
@@ -54,8 +48,19 @@ def merge_and_clean_mesh(mesh) -> tuple[np.ndarray, np.ndarray]:
     used = np.zeros(len(verts), dtype=bool)
     used[faces.reshape(-1)] = True
     remap = np.cumsum(used) - 1
-    verts, faces = verts[used], remap[faces]
+    return verts[used], remap[faces]
 
+
+def merge_and_clean_mesh(mesh) -> tuple[np.ndarray, np.ndarray]:
+    """Merge duplicate vertices and clean the topology of `mesh` in place (`clean_topology`'s rules) ->
+    (vertex_merge_map, pre_merge_faces).
+
+    vertex_merge_map (N_original,): for each original vertex, the index of the nearest merged vertex (cKDTree); as in the
+    reference every distance must be below 1e-6.  pre_merge_faces: a copy of the original (F_original, 3) faces."""
+    verts, faces = _arrays(mesh)
+    pre_merge_verts = verts.copy()
+    pre_merge_faces = np.array(mesh.faces, copy=True)
+    verts, faces = clean_topology(verts, faces)
     mesh.vertices = verts
     mesh.faces = faces
     distances, vertex_merge_map = cKDTree(verts).query(pre_merge_verts)

@@ -633,3 +633,157 @@ def gaussian_sample(params: torch.Tensor, eps: Optional[torch.Tensor] = None, *,
     _lib.check(rc, "amb_gaussian_sample")
     launch_count += 1
     return z
+
+
+# ---- anchor-mesh post-processing: quadric edge-collapse decimation and floater removal (csrc/mesh_process.cu) -------------
+NO_KEY = (1 << 64) - 1
+
+
+def mesh_scan_scratch(n_vertices: int, n_faces: int, device) -> tuple[torch.Tensor, torch.Tensor]:
+    """(work (V,) int32, scan scratch for max(V, F) items) shared by the mesh_* calls on one mesh."""
+    return torch.empty(max(n_vertices, 1), dtype=torch.int32, device=device), _scan_scratch(max(n_vertices, n_faces), device)
+
+
+def _scan_total(scan: torch.Tensor, n_items: int) -> int:
+    nints = C.c_int64()
+    _lib.check(_lib.load_library().amb_scan_scratch_ints(int(n_items), C.byref(nints)), "amb_scan_scratch_ints")
+    return int(scan[nints.value - 1].item())
+
+
+def _mesh_faces(faces: torch.Tensor) -> int:
+    _need(faces, torch.int32, "faces")
+    assert faces.dim() == 2 and faces.shape[1] == 3 and faces.is_contiguous(), "faces: expected a contiguous (F, 3) tensor"
+    return faces.shape[0]
+
+
+def mesh_adjacency(faces: torch.Tensor, n_vertices: int, work: torch.Tensor, scan: torch.Tensor):
+    """Vertex -> face CSR of (F, 3) int32 faces (F >= 1) and the edge list -> (vf_offsets (V+1), vf_faces (3F), neighbours (6F),
+    edges (E, 5) int32 = a < b, face count, f0, f1 ordered by (a, b), flags (V) uint8: 1 boundary, 2 non-manifold).
+    Reads E back (one sync)."""
+    global launch_count
+    F = _mesh_faces(faces)
+    dev = faces.device
+    lib = _lib.load_library()
+    off = torch.empty(n_vertices + 1, dtype=torch.int32, device=dev)
+    vf = torch.empty(3 * F, dtype=torch.int32, device=dev)
+    nb = torch.empty(6 * F, dtype=torch.int32, device=dev)
+    _lib.check(lib.amb_mesh_adjacency(faces.data_ptr(), F, n_vertices, work.data_ptr(), scan.data_ptr(), off.data_ptr(),
+                                      vf.data_ptr(), nb.data_ptr(), _stream()), "amb_mesh_adjacency")
+    E = _scan_total(scan, n_vertices)
+    edges = torch.empty(max(E, 1), 5, dtype=torch.int32, device=dev)
+    flags = torch.empty(max(n_vertices, 1), dtype=torch.uint8, device=dev)
+    _lib.check(lib.amb_mesh_edges(faces.data_ptr(), F, n_vertices, off.data_ptr(), vf.data_ptr(), nb.data_ptr(), work.data_ptr(),
+                                  scan.data_ptr(), edges.data_ptr(), flags.data_ptr(), _stream()), "amb_mesh_edges")
+    launch_count += 14
+    return off, vf, nb, edges[:E], flags
+
+
+def mesh_quadrics(positions: torch.Tensor, faces: torch.Tensor, adjacency) -> torch.Tensor:
+    """(V, 10) fp64 initial error quadrics: area-weighted face planes plus weighted boundary-edge planes."""
+    global launch_count
+    _need(positions, torch.float64, "positions")
+    _mesh_faces(faces)
+    off, vf, nb = adjacency[:3]
+    V = positions.shape[0]
+    q = torch.empty(V, 10, dtype=torch.float64, device=positions.device)
+    _lib.check(_lib.load_library().amb_mesh_quadrics(positions.data_ptr(), faces.data_ptr(), V, off.data_ptr(), vf.data_ptr(),
+                                                     nb.data_ptr(), q.data_ptr(), _stream()), "amb_mesh_quadrics")
+    launch_count += 1
+    return q
+
+
+def mesh_collapse_select(positions: torch.Tensor, quadrics: torch.Tensor, faces: torch.Tensor, adjacency):
+    """One round's independent set of cheapest valid collapses -> dict(keys (E,), targets (E, 3), vertex_min (2V,),
+    remap (V,), winners (n, 2) = (key, face count) unordered, removed = faces the winners remove).  Keys are uint64 bit
+    patterns held in int64 tensors.  Reads the winner count back (one sync)."""
+    global launch_count
+    _need(positions, torch.float64, "positions")
+    _need(quadrics, torch.float64, "quadrics")
+    off, vf, nb, edges, flags = adjacency
+    V, E, dev = positions.shape[0], edges.shape[0], positions.device
+    keys = torch.empty(max(E, 1), dtype=torch.int64, device=dev)
+    targets = torch.empty(max(E, 1), 3, dtype=torch.float64, device=dev)
+    vmin = torch.empty(2 * V, dtype=torch.int64, device=dev)
+    remap = torch.empty(V, dtype=torch.int32, device=dev)
+    counters = torch.empty(2, dtype=torch.int64, device=dev)
+    winners = torch.empty(max(E, 1), 2, dtype=torch.int64, device=dev)
+    _lib.check(_lib.load_library().amb_mesh_collapse_select(
+        positions.data_ptr(), quadrics.data_ptr(), faces.data_ptr(), V, off.data_ptr(), vf.data_ptr(), nb.data_ptr(),
+        edges.data_ptr(), E, flags.data_ptr(), keys.data_ptr(), targets.data_ptr(), vmin.data_ptr(), remap.data_ptr(),
+        counters.data_ptr(), winners.data_ptr(), _stream()), "amb_mesh_collapse_select")
+    n_win, removed = (int(v) for v in counters.tolist())
+    launch_count += 5
+    return dict(keys=keys, targets=targets, vertex_min=vmin, remap=remap, winners=winners[:n_win], removed=removed)
+
+
+def mesh_collapse_apply(edges: torch.Tensor, selection: dict, key_limit: int, positions: torch.Tensor,
+                        quadrics: torch.Tensor) -> torch.Tensor:
+    """Collapse every winner of `selection` whose key <= key_limit (b into a, a to its target, Q_a += Q_b), in place ->
+    the round's remap (V,) int32."""
+    global launch_count
+    _need(positions, torch.float64, "positions")
+    _need(quadrics, torch.float64, "quadrics")
+    s = selection
+    _lib.check(_lib.load_library().amb_mesh_collapse_apply(
+        edges.data_ptr(), edges.shape[0], positions.shape[0], s["keys"].data_ptr(), s["targets"].data_ptr(),
+        s["vertex_min"].data_ptr(), int(key_limit), s["remap"].data_ptr(), positions.data_ptr(), quadrics.data_ptr(), _stream()),
+        "amb_mesh_collapse_apply")
+    launch_count += 1
+    return s["remap"]
+
+
+def mesh_compact_faces(faces: torch.Tensor, scan: torch.Tensor, *, remap: Optional[torch.Tensor] = None,
+                       labels: Optional[torch.Tensor] = None, sizes: Optional[torch.Tensor] = None,
+                       min_size: int = 0) -> torch.Tensor:
+    """The faces, in order, whose corners (through `remap`) are distinct and, with `labels`, whose component has >= min_size
+    faces (`sizes[labels[f]]`) -> (F', 3) int32.  Reads F' back (one sync)."""
+    global launch_count
+    F = _mesh_faces(faces)
+    for t, nme in ((remap, "remap"), (labels, "labels"), (sizes, "sizes")):
+        if t is not None:
+            _need(t, torch.int32, nme)
+    out = torch.empty(max(F, 1), 3, dtype=torch.int32, device=faces.device)
+    _lib.check(_lib.load_library().amb_mesh_compact_faces(faces.data_ptr(), F, _ptr(remap), _ptr(labels), _ptr(sizes),
+                                                          int(min_size), scan.data_ptr(), out.data_ptr(), _stream()),
+               "amb_mesh_compact_faces")
+    launch_count += 3
+    return out[:_scan_total(scan, F) if F else 0]
+
+
+def mesh_compact_vertices(positions: torch.Tensor, faces: torch.Tensor, work: torch.Tensor,
+                          scan: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Drop unreferenced vertices, keeping the others in index order -> (positions (V', 3) fp64, faces renumbered).
+    Reads V' back (one sync)."""
+    global launch_count
+    _need(positions, torch.float64, "positions")
+    F = _mesh_faces(faces)
+    V = positions.shape[0]
+    out_p = torch.empty(max(V, 1), 3, dtype=torch.float64, device=positions.device)
+    out_f = torch.empty(max(F, 1), 3, dtype=torch.int32, device=positions.device)
+    _lib.check(_lib.load_library().amb_mesh_compact_vertices(positions.data_ptr(), V, faces.data_ptr(), F, work.data_ptr(),
+                                                             scan.data_ptr(), out_p.data_ptr(), out_f.data_ptr(), _stream()),
+               "amb_mesh_compact_vertices")
+    launch_count += 5
+    return out_p[:_scan_total(scan, V) if V else 0], out_f[:F]
+
+
+def mesh_face_components(edges: torch.Tensor, n_faces: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """Components of faces joined through edges held by exactly 2 faces -> (labels (F,) int32 = the smallest face index of
+    each face's component, sizes (F,) int32 = faces per label).  Union passes until stable (one sync each)."""
+    global launch_count
+    _need(edges, torch.int32, "edges")
+    lib = _lib.load_library()
+    labels = torch.empty(max(n_faces, 1), dtype=torch.int32, device=edges.device)
+    changed = torch.empty(1, dtype=torch.int32, device=edges.device)
+    first = 1
+    while True:
+        _lib.check(lib.amb_mesh_components(edges.data_ptr(), edges.shape[0], n_faces, first, labels.data_ptr(), changed.data_ptr(),
+                                           _stream()), "amb_mesh_components")
+        launch_count += 3
+        first = 0
+        if not int(changed.item()):
+            break
+    sizes = torch.empty_like(labels)
+    _lib.check(lib.amb_mesh_component_sizes(labels.data_ptr(), n_faces, sizes.data_ptr(), _stream()), "amb_mesh_component_sizes")
+    launch_count += 2
+    return labels[:n_faces], sizes[:n_faces]

@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define AMB_ABI_VERSION 16
+#define AMB_ABI_VERSION 17
 
 typedef void* amb_stream_t; /* cudaStream_t */
 
@@ -259,6 +259,55 @@ int amb_farthest_point_sample(const float* points, int batch, int n, int64_t ld,
                               int k, int64_t* out, amb_stream_t stream);
 int amb_gaussian_sample(const float* params, int64_t ld, int64_t rows, int channels, const float* eps, float* z,
                         float* logvar, float* std_out, amb_stream_t stream);
+
+/* ---- anchor-mesh post-processing: quadric edge-collapse decimation and floater removal (csrc/mesh_process.cu) -------------
+ * Replaces MeshPostprocessor.process_mesh's decimation and floater removal (actionmesh/preprocessing/mesh_processor.py:
+ * 104-161,288-325,374-425: trimesh simplify_quadric_decimation and split(only_watertight=False)).  The rules are in
+ * csrc/mesh_process.cu and DESIGN.md §15; actionmesh_b200/mesh_process.py drives the rounds.
+ * positions: (V, 3) fp64; faces: (F, 3) int32, three distinct indices in [0, V) (not checked on the device).  `scan` holds
+ * amb_scan_scratch_ints(max(V, F)) ints; `work` holds V ints.  Zero vertices or faces launch nothing (collapse_select still
+ * zeroes its counters).
+ *  mesh_adjacency: vf_offsets (V + 1) and vf_faces (3F): each vertex's faces in ascending order; neighbours (6F): per vertex
+ *    (from 2 * vf_offsets[v]) the other two corners of each of its faces, sorted.  Then counts the edges: afterwards
+ *    scan[amb_scan_scratch_ints(V) - 1] (device) is E.
+ *  mesh_edges (after mesh_adjacency, same scan; work receives each vertex's first edge): edges (E, 5) int32 = a < b, face count, and the (up to 2) faces holding the
+ *    edge in ascending order (-1 when absent or when more than 2 faces hold it), ordered by (a, b); flags (V) = bit 0 boundary
+ *    vertex, bit 1 vertex on a non-manifold edge.
+ *  mesh_quadrics: quadrics (V, 10) fp64, the upper triangle of each vertex's 4x4 error quadric row by row.
+ *  mesh_collapse_select: per edge its key (uint64; all ones when the collapse is invalid) and target (E, 3) fp64;
+ *    vertex_min (2V) uint64 = the minimum key at each vertex, then over its 1-ring; remap (V) = identity; counters (2) =
+ *    number of winning edges and the faces they would remove; winners (2E) = (key, face count) of each winner, unordered.
+ *  mesh_collapse_apply: every winner with key <= key_limit collapses b into a: remap[b] = a, a moves to its target,
+ *    Q_a += Q_b.
+ *  mesh_compact_faces: out_faces = the faces, in order, whose corners (through remap when given) are distinct and, when
+ *    labels is given, whose component has >= min_size faces (sizes[labels[f]]).  scan[last] (device) is their count.
+ *  mesh_compact_vertices: the referenced vertices in index order -> out_positions, and out_faces = faces renumbered;
+ *    scan[amb_scan_scratch_ints(V) - 1] (device) is their count.
+ *  mesh_components: one union pass over the edges with exactly 2 faces (first != 0 initialises labels (F) to 0..F-1); *changed
+ *    (device) is 0 once labels are final, each then the smallest face index of its edge-connected component.
+ *  mesh_component_sizes: sizes (F) = number of faces carrying each label. */
+int amb_mesh_adjacency(const int32_t* faces, int64_t n_faces, int64_t n_vertices, int32_t* work, int32_t* scan,
+                       int32_t* vf_offsets, int32_t* vf_faces, int32_t* neighbours, amb_stream_t stream);
+int amb_mesh_edges(const int32_t* faces, int64_t n_faces, int64_t n_vertices, const int32_t* vf_offsets,
+                   const int32_t* vf_faces, const int32_t* neighbours, int32_t* work, const int32_t* scan, int32_t* edges,
+                   uint8_t* flags, amb_stream_t stream);
+int amb_mesh_quadrics(const double* positions, const int32_t* faces, int64_t n_vertices, const int32_t* vf_offsets,
+                      const int32_t* vf_faces, const int32_t* neighbours, double* quadrics, amb_stream_t stream);
+int amb_mesh_collapse_select(const double* positions, const double* quadrics, const int32_t* faces, int64_t n_vertices,
+                             const int32_t* vf_offsets, const int32_t* vf_faces, const int32_t* neighbours,
+                             const int32_t* edges, int64_t n_edges, const uint8_t* flags, uint64_t* keys, double* targets,
+                             uint64_t* vertex_min, int32_t* remap, uint64_t* counters, uint64_t* winners,
+                             amb_stream_t stream);
+int amb_mesh_collapse_apply(const int32_t* edges, int64_t n_edges, int64_t n_vertices, const uint64_t* keys,
+                            const double* targets, const uint64_t* vertex_min, uint64_t key_limit, int32_t* remap,
+                            double* positions, double* quadrics, amb_stream_t stream);
+int amb_mesh_compact_faces(const int32_t* faces, int64_t n_faces, const int32_t* remap, const int32_t* labels,
+                           const int32_t* sizes, int min_size, int32_t* scan, int32_t* out_faces, amb_stream_t stream);
+int amb_mesh_compact_vertices(const double* positions, int64_t n_vertices, const int32_t* faces, int64_t n_faces,
+                              int32_t* work, int32_t* scan, double* out_positions, int32_t* out_faces, amb_stream_t stream);
+int amb_mesh_components(const int32_t* edges, int64_t n_edges, int64_t n_faces, int first, int32_t* labels, int32_t* changed,
+                        amb_stream_t stream);
+int amb_mesh_component_sizes(const int32_t* labels, int64_t n_faces, int32_t* sizes, amb_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -449,10 +449,75 @@ def group_vae_encode(res):
     res["reference_recipe_encoder"] = {"ms": ms, "tflops": flop / ms / 1e9}
 
 
+def group_mesh_process(res):
+    """Anchor-mesh post-processing at Stage 0's size: depth-9 sphere and torus from refine_octree + mesh_from_grid; host clean,
+    GPU decimation to 40 000 faces (with its round count) and floater removal (threshold 0.02), each timed with a host clock
+    around synchronised calls (second of two runs).  Then the Stage-II vertex-query block (full-width random weights, one
+    16-frame window, one target) at the undecimated and the decimated vertex count: the whole autoencoder call, and the
+    CUDA-event time of the query block's GEMMs (tag s2_q).  fast_simplification is not installed and not timed."""
+    import numpy as np
+    import torch
+
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import triposg_vae_ref as ref
+    from actionmesh_b200 import ops
+    from actionmesh_b200.autoencoder import AutoencoderConfig, B200Autoencoder
+    from actionmesh_b200.mesh_input import clean_topology
+    from actionmesh_b200.mesh_process import decimate, remove_floaters
+    from actionmesh_b200.triposg_vae import mesh_from_grid, refine_octree
+
+    res["card"] = _card()
+    counts = {}
+    for name, field in (("sphere", ref.sphere), ("torus", ref.torus)):
+        v, f = mesh_from_grid(refine_octree(field, ref.BOUNDS, 9), ref.BOUNDS, 9)
+        r = {}
+        for _ in range(2):
+            t0 = time.time()
+            v0, f0 = clean_topology(v.astype(np.float64), f.astype(np.int64))
+            t1 = time.time()
+            pos = torch.from_numpy(v0).cuda()
+            ft = torch.from_numpy(f0.astype(np.int32)).cuda()
+            work, scan = ops.mesh_scan_scratch(len(v0), len(f0), "cuda")
+            torch.cuda.synchronize()
+            t2 = time.time()
+            pos, ft, rounds = decimate(pos, ft, 40000, work, scan)
+            torch.cuda.synchronize()
+            t3 = time.time()
+            pos2, ft2 = remove_floaters(pos, ft, 0.02, work, scan)
+            torch.cuda.synchronize()
+            t4 = time.time()
+            r = {"vertices_in": len(v0), "faces_in": len(f0), "clean_ms": (t1 - t0) * 1e3, "decimate_ms": (t3 - t2) * 1e3,
+                 "rounds": rounds, "faces_out": int(ft.shape[0]), "vertices_out": int(pos.shape[0]),
+                 "floaters_ms": (t4 - t3) * 1e3, "faces_after_floaters": int(ft2.shape[0])}
+        res[f"{name}_depth9"] = r
+        counts[name] = (r["vertices_in"], r["vertices_out"])
+    ae = B200Autoencoder(AutoencoderConfig()).to("cuda")
+    ae.init_random_(seed=3)
+    g = torch.Generator().manual_seed(0)
+    T, N = 16, 2048
+    lat = torch.randn(1, T, N, 64, generator=g).cuda()
+    fs = torch.arange(T, dtype=torch.float32)[None]
+    src, tgt = torch.zeros(1), torch.full((1, 1), 0.5)
+    for label, V in (("undecimated", counts["sphere"][0]), ("decimated", counts["sphere"][1])):
+        q = torch.randn(1, V, 6, generator=g)
+        q[..., 3:] = torch.nn.functional.normalize(q[..., 3:], dim=-1)
+        q = q.cuda()
+        ae(latent=lat, framestep=fs, source_alpha=src, target_alphas=tgt, query=q)
+        torch.cuda.synchronize()
+        ops.event_log, ops.event_tags = [], {"s2_q"}
+        t0 = time.time()
+        ae(latent=lat, framestep=fs, source_alpha=src, target_alphas=tgt, query=q)
+        torch.cuda.synchronize()
+        ms = (time.time() - t0) * 1e3
+        qms = sum(e0.elapsed_time(e1) for _, e0, e1, _ in ops.event_log)
+        ops.event_log, ops.event_tags = None, set()
+        res[f"stage2_{label}"] = {"vertices": V, "autoencoder_call_ms": ms, "query_gemm_ms": qms}
+
+
 GROUPS = {
     "elementwise": group_elementwise, "gemm": group_gemm, "attn": group_attn, "attn_more": group_attn_more,
     "gemm_perf": group_gemm_perf, "attn_perf": group_attn_perf, "vae_decode": group_vae_decode,
-    "vae_encode": group_vae_encode,
+    "vae_encode": group_vae_encode, "mesh_process": group_mesh_process,
 }
 TAG = os.environ.get("AMB_PROBE_TAG", "")
 if os.environ.get("AMB_PROBE_LIB"):  # bring-up only: probe an experimental build (tools/build_variant.sh) instead of the product library
