@@ -1,6 +1,8 @@
-"""Kernel parity on the GPU (-m gpu): every C-ABI compute entry point against a torch fp32 reference of the same op
-on seeded inputs.  Tolerances: outputs are bf16, so relative Frobenius error <= 4e-3 (bf16 has 8 mantissa bits,
-2^-9 = 1.95e-3 per rounding; two roundings on the fused paths) unless the output is fp32 (1e-5)."""
+"""Kernel parity on the GPU (-m gpu): the GEMM, flash attention and the elementwise group of tools/gpu_probe.py against a
+torch fp32 reference of the same op on seeded inputs.  Tolerances: outputs are bf16, so relative Frobenius error <= 4e-3
+(bf16 has 8 mantissa bits, 2^-9 = 1.95e-3 per rounding; two roundings on the fused paths) unless the output is fp32
+(1e-5).  A norm over the whole output cannot see a single wrong row or a small bias: the element-by-element checks of the
+GEMM and attention are in test_kernel_exactness_gpu.py, and the remaining entry points are in test_entry_points_gpu.py."""
 import math
 import os
 import sys
@@ -104,6 +106,9 @@ def test_gemm_is_linear_in_a(probe):
     ("pair_clean_ragged", (2, 2, 300, 128 * 50 + 17, 128), {}),
     # one key far above every other: the running maximum jumps on that key's tile and the output is v of that key
     ("pair_single_spike_key", (1, 2, 300, 128 * 50, 128), dict(mode="spike")),
+    ("am_q129_k129", (1, 3, 129, 129, 128), {}),
+    ("am_chunks8_64keys", (1, 2, 64, 8 * 64, 128), dict(kv_chunks=8)),     # every tile is a ragged tail tile
+    ("am_chunks4_200keys", (2, 2, 300, 4 * 200, 128), dict(kv_chunks=4)),
 ])
 def test_flash_attention(probe, name, args, kw):
     res = {}
