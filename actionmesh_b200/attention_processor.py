@@ -19,7 +19,7 @@ import torch
 
 from . import ops
 from ._lib import AmbError
-from .denoiser import repack_cross_kv, repack_self_qkv
+from .blocks import repack_cross_kv, repack_self_qkv
 
 
 class B200AttentionProcessor:

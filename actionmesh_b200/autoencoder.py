@@ -21,17 +21,17 @@ There is no torch arithmetic on the path (torch owns buffers and does two memcpy
 """
 from __future__ import annotations
 
-import json
 import math
-import os
 from dataclasses import dataclass
 from typing import Callable, Optional
 
 import torch
 
 from . import ops
+from . import blocks
 from ._lib import AmbError
-from .denoiser import repack_cross_kv, repack_self_qkv
+from .blocks import SyntheticWeights, V, W, pack_block, repack_cross_kv
+from .module import B200Module
 
 
 @dataclass
@@ -62,7 +62,8 @@ def _pad64(n: int) -> int:
     return (n + 63) // 64 * 64
 
 
-class B200Autoencoder:
+class B200Autoencoder(B200Module):
+    config_class = AutoencoderConfig
     QUERY_CHUNK = 16384  # vertex rows per score-matrix chunk (S chunk = 16384 x 32832 fp32 = 2.2 GB at the default shape)
 
     def __init__(self, config: Optional[AutoencoderConfig] = None, **kwargs):
@@ -74,63 +75,15 @@ class B200Autoencoder:
             raise AmbError(f"unsupported width {c.width}")
         if c.in_channels != 3:
             raise AmbError("query points must be 3-D")
-        self._device = torch.device("cpu")
-        self._w: dict = {}
-        self._loaded = False
+        super().__init__()
         self.verbose = False
         self.prediction_mode = c.prediction_mode
 
-    # ------------------------------------------------------------------ nn.Module-like surface
-    @property
-    def device(self) -> torch.device:
-        return self._device
-
-    def eval(self):
-        return self
-
-    def to(self, device):
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise AmbError("B200Autoencoder only runs on a CUDA (sm_90) device; there is no CPU path")
-        if self._loaded and device != self._device:
-            self._w = {k: v.to(device) for k, v in self._w.items()}
-        self._device = device
-        return self
-
-    @classmethod
-    def from_pretrained(cls, path: str, device="cuda") -> "B200Autoencoder":
-        """Mirror of ActionMeshAutoencoder.from_pretrained(f"{dir}/autoencoder") (pipeline.py:193-197)."""
-        cfg_path = os.path.join(path, "config.json")
-        kwargs = {}
-        if os.path.exists(cfg_path):
-            raw = json.load(open(cfg_path))
-            kwargs = {k: v for k, v in raw.items() if k in AutoencoderConfig.__dataclass_fields__}
-        model = cls(AutoencoderConfig(**kwargs))
-        st = os.path.join(path, "model.safetensors")
-        if os.path.exists(st):
-            from safetensors.torch import load_file
-            sd = load_file(st)
-        else:
-            sd = torch.load(os.path.join(path, "pytorch_model.bin"), map_location="cpu")
-        model.to(device)
-        model.load_state_dict(sd)
-        return model
-
-    @ops.on_device
-    def load_state_dict(self, sd: dict) -> None:
+    def _pack_state_dict(self, sd: dict, dev: torch.device) -> dict:
         """Pack the reference's state dict: trunk GEMM weights bf16 (QKV fused + head-permuted); the fp32 query-path
         weights as split-bf16 [hi | hi | lo] operands; biases / norm weights fp32."""
         c = self.config
-        dev = self._device
-        if dev.type != "cuda":
-            raise AmbError("call .to('cuda') before load_state_dict")
         H, D = c.num_attention_heads, c.width
-
-        def f32(name):
-            return sd[name].detach().to(device=dev, dtype=torch.float32).contiguous()
-
-        def W(name):
-            return f32(name).to(torch.bfloat16).contiguous()
 
         def S3(t: torch.Tensor, kpad: Optional[int] = None, npad: Optional[int] = None) -> torch.Tensor:
             """fp32 (n, k) weight -> bf16 (npad, 3*kpad) [hi | hi | lo] via the split kernel."""
@@ -140,17 +93,11 @@ class B200Autoencoder:
             src[:n, :k].copy_(t)
             return ops.split3(src, torch.empty(np_, 3 * kp, dtype=torch.bfloat16, device=dev), weight=True)
 
+        f32 = lambda name: V(sd[name], dev)
         w = {}
-        w["post_quant.w"], w["post_quant.b"] = W("post_quant.weight"), f32("post_quant.bias")
+        w["post_quant.w"], w["post_quant.b"] = W(sd["post_quant.weight"], dev), f32("post_quant.bias")
         for i in range(c.num_layers):
-            p = f"blocks.{i}."
-            for n in ("norm_s_attn", "norm_ff"):
-                w[p + n + ".g"], w[p + n + ".b"] = f32(p + n + ".weight"), f32(p + n + ".bias")
-            w[p + "s.qkv"] = repack_self_qkv(f32(p + "s_attn.to_q.weight"), f32(p + "s_attn.to_k.weight"),
-                                             f32(p + "s_attn.to_v.weight"), H).to(torch.bfloat16).contiguous()
-            w[p + "s.o.w"], w[p + "s.o.b"] = W(p + "s_attn.to_out.0.weight"), f32(p + "s_attn.to_out.0.bias")
-            w[p + "ff1.w"], w[p + "ff1.b"] = W(p + "ff.net.0.proj.weight"), f32(p + "ff.net.0.proj.bias")
-            w[p + "ff2.w"], w[p + "ff2.b"] = W(p + "ff.net.2.weight"), f32(p + "ff.net.2.bias")
+            pack_block(w, sd, f"blocks.{i}.", f"blocks.{i}.", H, dev)
         # ---- fp32-grade query path (temporal_autoencoder.py:143-161)
         p = f"blocks.{c.num_layers}."
         self._qpad = _pad64(c.query_dim)
@@ -171,45 +118,23 @@ class B200Autoencoder:
         b = torch.zeros(self._opad, dtype=torch.float32, device=dev)
         b[: c.out_dim].copy_(f32("proj_out.bias"))
         w["proj_out.b"] = b
-        self._w = w
-        self._loaded = True
+        return w
 
     @ops.on_device
     def init_random_(self, seed: int = 1236) -> None:
         """Synthetic weights for benchmarks (no checkpoints offline): torch default Linear/LayerNorm inits, residual-branch
         output projections scaled by 1/sqrt(num_layers + 1), generated on the GPU."""
         c = self.config
-        dev = self._device
-        g = torch.Generator(device=dev).manual_seed(seed)
-        rs = 1.0 / math.sqrt(c.num_layers + 1)
         D = c.width
-
-        def lin(out_f, in_f, scale=1.0, bias=True):
-            bound = 1.0 / math.sqrt(in_f)
-            wt = (torch.rand(out_f, in_f, generator=g, device=dev) * 2 - 1) * bound * scale
-            bs = (torch.rand(out_f, generator=g, device=dev) * 2 - 1) * bound * scale if bias else None
-            return wt, bs
-
-        def ln(name):
-            sd[name + ".weight"], sd[name + ".bias"] = torch.ones(D, device=dev), torch.zeros(D, device=dev)
-
-        sd = {}
-        sd["post_quant.weight"], sd["post_quant.bias"] = lin(D, c.latent_channels)
-        sd["proj_query.weight"], sd["proj_query.bias"] = lin(D, c.query_dim)
-        sd["proj_out.weight"], sd["proj_out.bias"] = lin(c.out_dim, D)
-        ln("norm_out")
+        sd = SyntheticWeights(seed, self._device)
+        sd.linear("post_quant", D, c.latent_channels)
+        sd.linear("proj_query", D, c.query_dim)
+        sd.linear("proj_out", c.out_dim, D)
+        sd.layernorm("norm_out", D)
         for i in range(c.num_layers + 1):
-            p = f"blocks.{i}."
-            a = "x_attn" if i == c.num_layers else "s_attn"
-            ln(p + ("norm_x_attn" if i == c.num_layers else "norm_s_attn"))
-            ln(p + "norm_ff")
-            if i == c.num_layers:
-                ln(p + "x_attn.norm_cross")
-            for n in ("to_q", "to_k", "to_v"):
-                sd[p + f"{a}.{n}.weight"], _ = lin(D, D, bias=False)
-            sd[p + f"{a}.to_out.0.weight"], sd[p + f"{a}.to_out.0.bias"] = lin(D, D, scale=rs)
-            sd[p + "ff.net.0.proj.weight"], sd[p + "ff.net.0.proj.bias"] = lin(4 * D, D)
-            sd[p + "ff.net.2.weight"], sd[p + "ff.net.2.bias"] = lin(D, 4 * D, scale=rs)
+            query = i == c.num_layers
+            sd.dit_block(f"blocks.{i}.", D, 4 * D, 1.0 / math.sqrt(c.num_layers + 1), ("x_attn" if query else "s_attn",),
+                         norm_cross=query)
         self.load_state_dict(sd)
 
     # ------------------------------------------------------------------ reference helper (temporal_autoencoder.py:118-141)
@@ -231,8 +156,7 @@ class B200Autoencoder:
                 step_callback: Optional[Callable[[int, int], None]] = None) -> torch.Tensor:
         """temporal_autoencoder.py:163-269.  latent (B,T,N,C), framestep (B,T) [any device], source_alpha (B,),
         target_alphas (B,T_out), query (B,V,3|6) -> displacement field (B,T_out,V,out_dim) fp32 in [-1,1]."""
-        if not self._loaded:
-            raise AmbError("B200Autoencoder: weights not loaded")
+        self._check_loaded()
         assert target_alphas.ndim == 2 and source_alpha.ndim == 1
         c, w, dev = self.config, self._w, self._device
         B, T, N, C = latent.shape
@@ -292,17 +216,9 @@ class B200Autoencoder:
                 h.copy_(lat_proj)
                 ops.alpha_rows(src_a[b], tgt_a[b][i], D // 2, h.view(T, L, D)[:, N, :])
                 for l in range(c.num_layers):
-                    p = f"blocks.{l}."
-                    ops.layernorm(h, w[p + "norm_s_attn.g"], w[p + "norm_s_attn.b"], 1e-5, out=xn)
-                    ops.gemm(xn, w[p + "s.qkv"], qkv, norm=rope, tag="s2_gemm")
-                    q4 = qkv[:, 0:D].view(1, R, H, dh)
-                    k4 = qkv[:, D:2 * D].view(1, R, H, dh)
-                    v4 = qkv[:, 2 * D:3 * D].view(1, R, H, dh)
-                    ops.flash_attn(q4, k4, v4, att.view(1, R, H, dh), scale, tag="s2_attn")
-                    ops.gemm(att, w[p + "s.o.w"], h, bias=w[p + "s.o.b"], residual=h, tag="s2_gemm")
-                    ops.layernorm(h, w[p + "norm_ff.g"], w[p + "norm_ff.b"], 1e-5, out=xn)
-                    ops.gemm(xn, w[p + "ff1.w"], ff, bias=w[p + "ff1.b"], act=1, tag="s2_gemm")
-                    ops.gemm(ff, w[p + "ff2.w"], h, bias=w[p + "ff2.b"], residual=h, tag="s2_gemm")
+                    blocks.attention_half(w, f"blocks.{l}.", h, xn, qkv, att, (1, R), H, norm=rope, tag="s2_gemm",
+                                          attn_tag="s2_attn")
+                    blocks.output_half(w, f"blocks.{l}.", "s", h, att, xn, ff, tag="s2_gemm")
                 # ---- K, V^T of the query cross-attention from the trunk output (norm_cross = layer_norm, :101)
                 ops.layernorm(h, w[pq + "norm_cross.g"], w[pq + "norm_cross.b"], 1e-5, out=ctx32)
                 ops.split3(ctx32, ctx3)                                        # writes rows [0, R); pad rows remain 0

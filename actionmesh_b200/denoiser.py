@@ -19,9 +19,7 @@ scheduler threads through its loop, scheduler.py:204,224-232).
 """
 from __future__ import annotations
 
-import json
 import math
-import os
 from dataclasses import dataclass, field
 from typing import Optional
 
@@ -29,6 +27,9 @@ import torch
 
 from . import ops
 from ._lib import AmbError
+from .blocks import SyntheticWeights, V, W, pack_block
+from .blocks import repack_cross_kv, repack_self_qkv  # noqa: F401  (also importable from here, where callers import them)
+from .module import B200Module
 
 
 @dataclass
@@ -53,27 +54,6 @@ class DenoiserConfig:
         return int(self.width * self.mlp_ratio)
 
 
-def repack_self_qkv(wq: torch.Tensor, wk: torch.Tensor, wv: torch.Tensor, heads: int) -> torch.Tensor:
-    """Head-interleaved split of attention_processor.py:106-110 folded into the weights (SURVEY A.2).
-
-    The reference takes head h's q/k/v from columns [3dh, 3d(h+1)) of cat(q,k,v).  Selecting the matching ROWS of
-    cat(Wq,Wk,Wv) once gives a standard fused QKV GEMM whose output is [Q(h,d) | K(h,d) | V(h,d)]."""
-    wcat = torch.cat([wq, wk, wv], dim=0)  # (3*inner, in)
-    inner = wq.shape[0]
-    dh = inner // heads
-    wcat = wcat.view(heads, 3, dh, -1)
-    return torch.cat([wcat[:, 0].reshape(inner, -1), wcat[:, 1].reshape(inner, -1), wcat[:, 2].reshape(inner, -1)], 0)
-
-
-def repack_cross_kv(wk: torch.Tensor, wv: torch.Tensor, heads: int) -> torch.Tensor:
-    """Same for the cross-attention [k|v] split (attention_processor.py:111-115); q keeps the plain head view (:117)."""
-    wcat = torch.cat([wk, wv], dim=0)
-    inner = wk.shape[0]
-    dh = inner // heads
-    wcat = wcat.view(heads, 2, dh, -1)
-    return torch.cat([wcat[:, 0].reshape(inner, -1), wcat[:, 1].reshape(inner, -1)], 0)
-
-
 class WindowState:
     """Opaque per-window cache returned in the `freqs_rot` slot: RoPE tables + context K/V of every layer."""
 
@@ -86,8 +66,10 @@ class WindowState:
         self.source = None                              # identity of the (context, framestep) this state was built from
 
 
-class B200Denoiser:
+class B200Denoiser(B200Module):
     """Drop-in for ActionMeshDenoiser on the Stage-I hot path (inference only)."""
+
+    config_class = DenoiserConfig
 
     def __init__(self, config: Optional[DenoiserConfig] = None, residual_fp32: bool = True, **kwargs):
         """`residual_fp32`: keep the residual stream (and the LayerNorm inputs) in fp32 instead of the bf16 the
@@ -101,52 +83,13 @@ class B200Denoiser:
             raise AmbError(f"B200Denoiser: head_dim must be 128 (width {c.width} / heads {c.num_attention_heads})")
         if c.width % 256 or c.in_channels % 64 or c.cross_attention_dim % 64:
             raise AmbError("B200Denoiser: width must be a multiple of 256, in_channels/cross_attention_dim of 64")
+        super().__init__()
         self.out_channels = c.in_channels
-        self._device = torch.device("cpu")
-        self._w: dict = {}          # packed device weights
         self._ws: dict = {}         # workspaces keyed by (B, T, N)
-        self._loaded = False
 
-    # ------------------------------------------------------------------ nn.Module-like surface used by the pipeline
-    @property
-    def device(self) -> torch.device:
-        return self._device
-
-    def eval(self):
-        return self
-
-    def to(self, device):
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise AmbError("B200Denoiser runs on CUDA (sm_90a) only; there is no CPU fallback")
-        if device.index is None:
-            device = torch.device("cuda", torch.cuda.current_device())
-        if self._loaded and self._device != device:
-            self._w = {k: v.to(device) for k, v in self._w.items()}
+    def _after_to(self, moved: bool) -> None:
+        if moved:
             self._ws = {}
-        self._device = device
-        return self
-
-    @classmethod
-    def from_pretrained(cls, path: str, device="cuda") -> "B200Denoiser":
-        """Mirror of PyTorchModelHubMixin.from_pretrained(f"{dir}/denoiser") (pipeline.py:180-182): config.json +
-        model.safetensors / pytorch_model.bin with the reference's state-dict keys."""
-        cfg_path = os.path.join(path, "config.json")
-        kwargs = {}
-        if os.path.exists(cfg_path):
-            raw = json.load(open(cfg_path))
-            fields = DenoiserConfig.__dataclass_fields__
-            kwargs = {k: (tuple(v) if isinstance(v, list) else v) for k, v in raw.items() if k in fields}
-        model = cls(DenoiserConfig(**kwargs))
-        st = os.path.join(path, "model.safetensors")
-        if os.path.exists(st):
-            from safetensors.torch import load_file
-            sd = load_file(st)
-        else:
-            sd = torch.load(os.path.join(path, "pytorch_model.bin"), map_location="cpu")
-        model.to(device)
-        model.load_state_dict(sd)
-        return model
 
     # ------------------------------------------------------------------ the 21 blocks as a launch program
     def _block_program(self, ws: dict, st: WindowState, b0: int, nb: int, B: int, T: int, N: int, shard):
@@ -249,50 +192,17 @@ class B200Denoiser:
         assert h_in is h  # the last block is never a pushing block: its output lives in ws['h'] for the output head
 
     # ------------------------------------------------------------------ weights
-    def load_state_dict(self, sd: dict) -> None:
-        """Pack the reference's state dict (keys of SURVEY A.1) into kernel-ready device tensors: GEMM weights bf16
-        (QKV / KV fused and head-permuted), biases / norm weights fp32."""
-        if self._device.type != "cuda":
-            raise AmbError("call .to('cuda') before load_state_dict")
-        with torch.cuda.device(self._device):
-            self._w = self._pack_state_dict(sd, self._device)
-        self._loaded = True
-
     def _pack_state_dict(self, sd: dict, dev: torch.device) -> dict:
-        c = self.config
-        H = c.num_attention_heads
-
-        def W(name):  # GEMM operand
-            return sd[name].detach().to(device=dev, dtype=torch.float32).to(torch.bfloat16).contiguous()
-
-        def V(name):  # fp32 vector
-            return sd[name].detach().to(device=dev, dtype=torch.float32).contiguous()
-
+        """Pack the reference's state dict (keys of SURVEY A.1) into kernel-ready tensors: GEMM weights bf16 (QKV / KV
+        fused and head-permuted), biases / norm weights fp32."""
         w = {}
-        w["proj_in.w"], w["proj_in.b"] = W("proj_in.weight"), V("proj_in.bias")
-        w["time1.w"], w["time1.b"] = W("time_proj.linear_1.weight"), V("time_proj.linear_1.bias")
-        w["time2.w"], w["time2.b"] = W("time_proj.linear_2.weight"), V("time_proj.linear_2.bias")
-        w["norm_out.g"], w["norm_out.b"] = V("norm_out.weight"), V("norm_out.bias")
-        w["proj_out.w"], w["proj_out.b"] = W("proj_out.weight"), V("proj_out.bias")
-        for i in range(c.num_layers):
-            p = f"blocks.{i}."
-            if i > c.num_layers // 2:
-                w[p + "skip.w"], w[p + "skip.b"] = W(p + "linear_skip.weight"), V(p + "linear_skip.bias")
-                w[p + "norm_skip.g"], w[p + "norm_skip.b"] = V(p + "norm_skip.weight"), V(p + "norm_skip.bias")
-            for n in ("norm_s_attn", "norm_x_attn", "norm_ff"):
-                w[p + n + ".g"], w[p + n + ".b"] = V(p + n + ".weight"), V(p + n + ".bias")
-            f32 = lambda k: sd[k].detach().to(device=dev, dtype=torch.float32)
-            w[p + "s.qkv"] = repack_self_qkv(f32(p + "s_attn.to_q.weight"), f32(p + "s_attn.to_k.weight"),
-                                             f32(p + "s_attn.to_v.weight"), H).to(torch.bfloat16).contiguous()
-            w[p + "s.nq"], w[p + "s.nk"] = V(p + "s_attn.norm_q.weight"), V(p + "s_attn.norm_k.weight")
-            w[p + "s.o.w"], w[p + "s.o.b"] = W(p + "s_attn.to_out.0.weight"), V(p + "s_attn.to_out.0.bias")
-            w[p + "x.q"] = W(p + "x_attn.to_q.weight")
-            w[p + "x.kv"] = repack_cross_kv(f32(p + "x_attn.to_k.weight"), f32(p + "x_attn.to_v.weight"),
-                                            H).to(torch.bfloat16).contiguous()
-            w[p + "x.nq"], w[p + "x.nk"] = V(p + "x_attn.norm_q.weight"), V(p + "x_attn.norm_k.weight")
-            w[p + "x.o.w"], w[p + "x.o.b"] = W(p + "x_attn.to_out.0.weight"), V(p + "x_attn.to_out.0.bias")
-            w[p + "ff1.w"], w[p + "ff1.b"] = W(p + "ff.net.0.proj.weight"), V(p + "ff.net.0.proj.bias")
-            w[p + "ff2.w"], w[p + "ff2.b"] = W(p + "ff.net.2.weight"), V(p + "ff.net.2.bias")
+        w["proj_in.w"], w["proj_in.b"] = W(sd["proj_in.weight"], dev), V(sd["proj_in.bias"], dev)
+        w["time1.w"], w["time1.b"] = W(sd["time_proj.linear_1.weight"], dev), V(sd["time_proj.linear_1.bias"], dev)
+        w["time2.w"], w["time2.b"] = W(sd["time_proj.linear_2.weight"], dev), V(sd["time_proj.linear_2.bias"], dev)
+        w["norm_out.g"], w["norm_out.b"] = V(sd["norm_out.weight"], dev), V(sd["norm_out.bias"], dev)
+        w["proj_out.w"], w["proj_out.b"] = W(sd["proj_out.weight"], dev), V(sd["proj_out.bias"], dev)
+        for i in range(self.config.num_layers):
+            pack_block(w, sd, f"blocks.{i}.", f"blocks.{i}.", self.config.num_attention_heads, dev)
         return w
 
     def init_random_(self, seed: int = 1234, residual_scale: Optional[float] = None) -> None:
@@ -300,42 +210,16 @@ class B200Denoiser:
         branch output projections scaled by 1/sqrt(num_layers) so activations stay O(1) (SURVEY 8(d)).  Generated
         directly on the GPU (no 5.8 GB host copy)."""
         c = self.config
-        g = torch.Generator(device=self._device).manual_seed(seed)
         rs = residual_scale if residual_scale is not None else 1.0 / math.sqrt(c.num_layers)
-
-        def lin(out_f, in_f, scale=1.0, bias=True):
-            bound = 1.0 / math.sqrt(in_f)
-            wt = (torch.rand(out_f, in_f, generator=g, device=self._device) * 2 - 1) * bound * scale
-            bs = (torch.rand(out_f, generator=g, device=self._device) * 2 - 1) * bound * scale if bias else None
-            return wt, bs
-
-        sd = {}
-        sd["proj_in.weight"], sd["proj_in.bias"] = lin(c.width, c.in_channels)
-        sd["time_proj.linear_1.weight"], sd["time_proj.linear_1.bias"] = lin(c.width * 4, c.width)
-        sd["time_proj.linear_2.weight"], sd["time_proj.linear_2.bias"] = lin(c.width, c.width * 4)
-        sd["norm_out.weight"] = torch.ones(c.width, device=self._device)
-        sd["norm_out.bias"] = torch.zeros(c.width, device=self._device)
-        sd["proj_out.weight"], sd["proj_out.bias"] = lin(c.in_channels, c.width)
+        sd = SyntheticWeights(seed, self._device)
+        sd.linear("proj_in", c.width, c.in_channels)
+        sd.linear("time_proj.linear_1", c.width * 4, c.width)
+        sd.linear("time_proj.linear_2", c.width, c.width * 4)
+        sd.layernorm("norm_out", c.width)
+        sd.linear("proj_out", c.in_channels, c.width)
         for i in range(c.num_layers):
-            p = f"blocks.{i}."
-            b = {}
-            if i > c.num_layers // 2:
-                b[p + "linear_skip.weight"], b[p + "linear_skip.bias"] = lin(c.width, 2 * c.width)
-                b[p + "norm_skip.weight"] = torch.ones(c.width, device=self._device)
-                b[p + "norm_skip.bias"] = torch.zeros(c.width, device=self._device)
-            for n in ("norm_s_attn", "norm_x_attn", "norm_ff"):
-                b[p + n + ".weight"] = torch.ones(c.width, device=self._device)
-                b[p + n + ".bias"] = torch.zeros(c.width, device=self._device)
-            for a, kd in (("s_attn", c.width), ("x_attn", c.cross_attention_dim)):
-                b[p + a + ".to_q.weight"], _ = lin(c.width, c.width, bias=False)
-                b[p + a + ".to_k.weight"], _ = lin(c.width, kd, bias=False)
-                b[p + a + ".to_v.weight"], _ = lin(c.width, kd, bias=False)
-                b[p + a + ".norm_q.weight"] = torch.ones(c.head_dim, device=self._device)
-                b[p + a + ".norm_k.weight"] = torch.ones(c.head_dim, device=self._device)
-                b[p + a + ".to_out.0.weight"], b[p + a + ".to_out.0.bias"] = lin(c.width, c.width, scale=rs)
-            b[p + "ff.net.0.proj.weight"], b[p + "ff.net.0.proj.bias"] = lin(c.ff_dim, c.width)
-            b[p + "ff.net.2.weight"], b[p + "ff.net.2.bias"] = lin(c.width, c.ff_dim, scale=rs)
-            sd.update(b)
+            sd.dit_block(f"blocks.{i}.", c.width, c.ff_dim, rs, ("s_attn", "x_attn"), cross_dim=c.cross_attention_dim,
+                         qk_norm=c.head_dim, skip=i > c.num_layers // 2)
         self.load_state_dict(sd)
         del sd
         torch.cuda.empty_cache()
@@ -416,6 +300,7 @@ class B200Denoiser:
         return st
 
     # ------------------------------------------------------------------ forward
+    @ops.on_device
     @torch.no_grad()
     def forward(self, hidden_states: torch.Tensor, context: torch.Tensor, framestep: torch.Tensor,
                 diffusion_time: torch.Tensor, mask: Optional[torch.Tensor] = None, freqs_rot=None):
@@ -423,12 +308,7 @@ class B200Denoiser:
 
         `freqs_rot` is the WindowState from a previous call of the same window (or None).  The prediction is a VIEW of a
         workspace buffer that the next forward() overwrites (the scheduler consumes it immediately); clone it to keep it."""
-        if not self._loaded:
-            raise AmbError("B200Denoiser: weights not loaded")
-        with torch.cuda.device(self._device):
-            return self._forward(hidden_states, context, framestep, diffusion_time, mask, freqs_rot)
-
-    def _forward(self, hidden_states, context, framestep, diffusion_time, mask, freqs_rot):
+        self._check_loaded()
         B, T, N, C = hidden_states.shape
         # The state caches the image conditioning as well as the RoPE tables, so (unlike the reference's freqs_rot) it is
         # only reused for the context / framestep it was built from.

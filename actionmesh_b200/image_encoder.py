@@ -27,8 +27,9 @@ from typing import List, Optional
 
 import torch
 
-from . import ops
+from . import blocks, ops
 from ._lib import AmbError
+from .module import B200Module, read_weights
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_STD = (0.229, 0.224, 0.225)
@@ -45,7 +46,7 @@ def default_preprocessor():
                              do_convert_rgb=True)
 
 
-class B200ImageEncoder:
+class B200ImageEncoder(B200Module):
     def __init__(self, pretrained_dino_feature_extractor: Optional[str] = None,
                  pretrained_dino_model: Optional[str] = None, *, hidden_size: int = 1024, num_layers: int = 24,
                  num_heads: int = 16, patch_size: int = 14, image_size: int = 224, mlp_ratio: int = 4,
@@ -57,9 +58,7 @@ class B200ImageEncoder:
         if precision not in ("fp32", "bf16"):
             raise AmbError("B200ImageEncoder: precision must be 'fp32' (reference-grade, default) or 'bf16'")
         self.precision = precision
-        self._device = torch.device("cpu")
-        self._w: dict = {}
-        self._loaded = False
+        super().__init__()
         self._pending_sd = None
         self.image_preprocess_dino = None
         self._gpu_preprocess = None
@@ -77,42 +76,20 @@ class B200ImageEncoder:
         if self.image_preprocess_dino is None:
             self.image_preprocess_dino = default_preprocessor()
         if pretrained_dino_model is not None:
-            from safetensors.torch import load_file
-            st = os.path.join(pretrained_dino_model, "model.safetensors")
-            self._pending_sd = load_file(st) if os.path.exists(st) else torch.load(
-                os.path.join(pretrained_dino_model, "pytorch_model.bin"), map_location="cpu")
+            self._pending_sd = read_weights(pretrained_dino_model, self.weight_files)
 
-    # ---- module-like surface
-    @property
-    def device(self) -> torch.device:
-        return self._device
-
-    def eval(self):
-        return self
-
-    def to(self, device):
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise AmbError("B200ImageEncoder runs on CUDA (sm_90a) only")
-        if device.index is None:
-            device = torch.device("cuda", torch.cuda.current_device())
-        self._device = device
+    def _after_to(self, moved: bool) -> None:
+        """The weights of `pretrained_dino_model` are packed on the first `to()`."""
         if self._pending_sd is not None:
             self.load_state_dict(self._pending_sd)
             self._pending_sd = None
-        elif self._loaded:
-            self._w = {k: v.to(device) for k, v in self._w.items()}
-        return self
 
     # ---- weights (HF Dinov2Model state-dict keys)
-    @ops.on_device
-    def load_state_dict(self, sd: dict) -> None:
-        dev = self._device
-        if dev.type != "cuda":
-            raise AmbError("call .to('cuda') before load_state_dict")
+    def _pack_state_dict(self, sd: dict, dev: torch.device) -> dict:
         sd = {k[len("dinov2."):] if k.startswith("dinov2.") else k: v for k, v in sd.items()}
         D, P = self.hidden_size, self.patch_size
         f32 = lambda k: sd[k].detach().to(device=dev, dtype=torch.float32)
+        V = lambda k: blocks.V(sd[k], dev)
         if self.precision == "fp32":   # split operand [hi | hi | lo] along K (ops.split3, weight layout)
             W = lambda t: ops.split3(t.contiguous(), torch.empty(t.shape[0], 3 * t.shape[1], dtype=torch.bfloat16, device=dev),
                                      weight=True)
@@ -137,19 +114,18 @@ class B200ImageEncoder:
         w["base"] = base.contiguous()
         for i in range(self.num_layers):
             p = f"encoder.layer.{i}."
-            w[p + "n1.g"], w[p + "n1.b"] = f32(p + "norm1.weight").contiguous(), f32(p + "norm1.bias").contiguous()
             a = p + "attention.attention."
-            w[p + "qkv.w"] = W(torch.cat([f32(a + "query.weight"), f32(a + "key.weight"), f32(a + "value.weight")], 0))
-            w[p + "qkv.b"] = torch.cat([f32(a + "query.bias"), f32(a + "key.bias"), f32(a + "value.bias")], 0).contiguous()
-            w[p + "o.w"], w[p + "o.b"] = W(f32(p + "attention.output.dense.weight")), f32(p + "attention.output.dense.bias").contiguous()
-            w[p + "ls1"] = f32(p + "layer_scale1.lambda1").contiguous()
-            w[p + "n2.g"], w[p + "n2.b"] = f32(p + "norm2.weight").contiguous(), f32(p + "norm2.bias").contiguous()
-            w[p + "fc1.w"], w[p + "fc1.b"] = W(f32(p + "mlp.fc1.weight")), f32(p + "mlp.fc1.bias").contiguous()
-            w[p + "fc2.w"], w[p + "fc2.b"] = W(f32(p + "mlp.fc2.weight")), f32(p + "mlp.fc2.bias").contiguous()
-            w[p + "ls2"] = f32(p + "layer_scale2.lambda1").contiguous()
-        w["ln.g"], w["ln.b"] = f32("layernorm.weight").contiguous(), f32("layernorm.bias").contiguous()
-        self._w = w
-        self._loaded = True
+            w[p + "norm_s_attn.g"], w[p + "norm_s_attn.b"] = V(p + "norm1.weight"), V(p + "norm1.bias")
+            w[p + "s.qkv"] = W(torch.cat([f32(a + "query.weight"), f32(a + "key.weight"), f32(a + "value.weight")], 0))
+            w[p + "s.qkv.b"] = torch.cat([f32(a + "query.bias"), f32(a + "key.bias"), f32(a + "value.bias")], 0).contiguous()
+            w[p + "s.o.w"], w[p + "s.o.b"] = W(f32(p + "attention.output.dense.weight")), V(p + "attention.output.dense.bias")
+            w[p + "ls1"] = V(p + "layer_scale1.lambda1")
+            w[p + "norm_ff.g"], w[p + "norm_ff.b"] = V(p + "norm2.weight"), V(p + "norm2.bias")
+            w[p + "ff1.w"], w[p + "ff1.b"] = W(f32(p + "mlp.fc1.weight")), V(p + "mlp.fc1.bias")
+            w[p + "ff2.w"], w[p + "ff2.b"] = W(f32(p + "mlp.fc2.weight")), V(p + "mlp.fc2.bias")
+            w[p + "ls2"] = V(p + "layer_scale2.lambda1")
+        w["ln.g"], w["ln.b"] = V("layernorm.weight"), V("layernorm.bias")
+        return w
 
     @ops.on_device
     def init_random_(self, seed: int = 1235) -> None:
@@ -194,8 +170,7 @@ class B200ImageEncoder:
     @torch.no_grad()
     def encode_pixel_values(self, pixel_values: torch.Tensor) -> torch.Tensor:
         """pixel_values (T,3,224,224) fp32 (host or device) -> last_hidden_state (T, 1+g*g, D) fp32."""
-        if not self._loaded:
-            raise AmbError("B200ImageEncoder: weights not loaded")
+        self._check_loaded()
         w = self._w
         dev = self._device
         px = pixel_values.to(device=dev, dtype=torch.float32).contiguous()
@@ -215,19 +190,11 @@ class B200ImageEncoder:
         qkv = torch.empty(M, 3 * D, dtype=bf, device=dev)
         att = torch.empty(M, D, dtype=bf, device=dev)
         hid = torch.empty(M, F_, dtype=bf, device=dev)
-        scale = 1.0 / math.sqrt(D // H)
         for i in range(self.num_layers):
             p = f"encoder.layer.{i}."
-            ops.layernorm(x, w[p + "n1.g"], w[p + "n1.b"], self.eps, out=xn)
-            ops.gemm(xn, w[p + "qkv.w"], qkv, bias=w[p + "qkv.b"])
-            q4 = qkv[:, 0:D].unflatten(0, (T, L)).unflatten(-1, (H, D // H))
-            k4 = qkv[:, D:2 * D].unflatten(0, (T, L)).unflatten(-1, (H, D // H))
-            v4 = qkv[:, 2 * D:].unflatten(0, (T, L)).unflatten(-1, (H, D // H))
-            ops.flash_attn(q4, k4, v4, att.view(T, L, H, D // H), scale, tag="attn_dino")
-            ops.gemm(att, w[p + "o.w"], x, bias=w[p + "o.b"], col_scale=w[p + "ls1"], residual=x)
-            ops.layernorm(x, w[p + "n2.g"], w[p + "n2.b"], self.eps, out=xn)
-            ops.gemm(xn, w[p + "fc1.w"], hid, bias=w[p + "fc1.b"], act=1)
-            ops.gemm(hid, w[p + "fc2.w"], x, bias=w[p + "fc2.b"], col_scale=w[p + "ls2"], residual=x)
+            blocks.attention_half(w, p, x, xn, qkv, att, (T, L), H, eps=self.eps, bias=w[p + "s.qkv.b"], tag="gemm",
+                                  attn_tag="attn_dino")
+            blocks.output_half(w, p, "s", x, att, xn, hid, eps=self.eps, layer_scale=(w[p + "ls1"], w[p + "ls2"]), tag="gemm")
         out = torch.empty(M, D, dtype=torch.float32, device=dev)
         ops.layernorm(x, w["ln.g"], w["ln.b"], self.eps, out=out)
         return out.view(T, L, D)
@@ -253,17 +220,17 @@ class B200ImageEncoder:
         scale = 1.0 / math.sqrt(D // H)
         for i in range(self.num_layers):
             p = f"encoder.layer.{i}."
-            ops.layernorm(x, w[p + "n1.g"], w[p + "n1.b"], self.eps, out=t32)
+            ops.layernorm(x, w[p + "norm_s_attn.g"], w[p + "norm_s_attn.b"], self.eps, out=t32)
             ops.split3(t32, a3)
-            ops.gemm(a3, w[p + "qkv.w"], qkv, bias=w[p + "qkv.b"])
+            ops.gemm(a3, w[p + "s.qkv"], qkv, bias=w[p + "s.qkv.b"])
             ops.attn_small_f32(qkv, T, L, H, scale, att, tag="attn_dino")
             ops.split3(att, a3)
-            ops.gemm(a3, w[p + "o.w"], x, bias=w[p + "o.b"], col_scale=w[p + "ls1"], residual=x)
-            ops.layernorm(x, w[p + "n2.g"], w[p + "n2.b"], self.eps, out=t32)
+            ops.gemm(a3, w[p + "s.o.w"], x, bias=w[p + "s.o.b"], col_scale=w[p + "ls1"], residual=x)
+            ops.layernorm(x, w[p + "norm_ff.g"], w[p + "norm_ff.b"], self.eps, out=t32)
             ops.split3(t32, a3)
-            ops.gemm(a3, w[p + "fc1.w"], hid, bias=w[p + "fc1.b"], act=1)
+            ops.gemm(a3, w[p + "ff1.w"], hid, bias=w[p + "ff1.b"], act=1)
             ops.split3(hid, h3)
-            ops.gemm(h3, w[p + "fc2.w"], x, bias=w[p + "fc2.b"], col_scale=w[p + "ls2"], residual=x)
+            ops.gemm(h3, w[p + "ff2.w"], x, bias=w[p + "ff2.b"], col_scale=w[p + "ls2"], residual=x)
         out = torch.empty(M, D, dtype=f32, device=dev)
         ops.layernorm(x, w["ln.g"], w["ln.b"], self.eps, out=out)
         return out.view(T, L, D)

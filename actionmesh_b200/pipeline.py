@@ -239,6 +239,18 @@ def _vertex_normals(vertices: torch.Tensor, faces: torch.Tensor) -> torch.Tensor
     return vn / vn.norm(dim=-1, keepdim=True).clamp_min(1e-12)
 
 
+def vertex_normals(verts: torch.Tensor, faces: torch.Tensor) -> torch.Tensor:
+    """(V, 3) fp32 unit vertex normals: trimesh's `vertex_normals`, the reference's source (mesh_processor.py:98), or
+    `_vertex_normals` when trimesh is not installed."""
+    try:
+        import trimesh
+
+        return torch.as_tensor(trimesh.Trimesh(vertices=verts.cpu().numpy(), faces=faces.cpu().numpy(),
+                                               process=False).vertex_normals.copy(), dtype=torch.float32)
+    except ImportError:
+        return _vertex_normals(verts.to(torch.float32), faces.to(verts.device))
+
+
 class ActionMeshB200Pipeline:
     """Drop-in for `ActionMeshPipeline` on the CUDA path: same constructor arguments, `.to(device)`, and `__call__`
     signature / return value (reference actionmesh/pipeline.py:47-53,205,602-685).
@@ -312,6 +324,27 @@ class ActionMeshB200Pipeline:
         return self._target_device
 
     # ---- stages
+    def _apply_overrides(self, input, stage_0_steps, face_decimation, floaters_threshold, stage_1_steps, guidance_scales,
+                         anchor_idx) -> None:
+        """The per-call overrides of `__call__` (pipeline.py:637-656), then background removal and image processing of
+        the frames."""
+        if stage_0_steps is not None:
+            self.cfg.model.image_to_3D_denoiser.num_inference_steps = stage_0_steps
+        if stage_1_steps is not None:
+            self.scheduler.num_inference_steps = stage_1_steps
+        if guidance_scales is not None:
+            self.cf_guidance.guidance_scales = guidance_scales
+        if face_decimation is not None:
+            self.mesh_process.face_decimation = face_decimation
+        if floaters_threshold is not None:
+            self.mesh_process.floaters_threshold = floaters_threshold
+        if anchor_idx is not None:
+            self.cfg.anchor_idx = anchor_idx
+        if self.background_removal is not None:
+            input.frames = self.background_removal.process_images(input.frames)
+        if self.image_process is not None:
+            input.frames = self.image_process.process_images(input.frames)
+
     def init_banks_from_anchor(self, input, seed: int = 44):
         """Stage 0 through the injected image-to-3D component (pipeline.py:387-433) -> (LatentBank, anchor mesh)."""
         if self.image_to_3d_pipe is None:
@@ -330,17 +363,7 @@ class ActionMeshB200Pipeline:
 
     def _stage_pipeline(self) -> "AnimationPipeline":
         faces_holder = {}
-
-        def normals_fn(verts: torch.Tensor) -> torch.Tensor:
-            faces = faces_holder["faces"]
-            try:
-                import trimesh  # the reference's source of vertex normals
-
-                return torch.as_tensor(trimesh.Trimesh(vertices=verts.cpu().numpy(), faces=faces.cpu().numpy(),
-                                                       process=False).vertex_normals.copy(), dtype=torch.float32)
-            except ImportError:
-                return _vertex_normals(verts.to(torch.float32), faces.to(verts.device))
-
+        normals_fn = lambda verts: vertex_normals(verts, faces_holder["faces"])
         pipe = AnimationPipeline(self.temporal_3D_denoiser, self.scheduler, self.cf_guidance, self.temporal_3D_vae,
                                  self.image_encoder, sliding_window_autoencoder=self.cfg.sliding_window_autoencoder,
                                  subsampling_level=self.cfg.subsampling_level, normals_fn=normals_fn,
@@ -355,23 +378,8 @@ class ActionMeshB200Pipeline:
                  floaters_threshold: Optional[float] = None, stage_1_steps: Optional[int] = None,
                  guidance_scales: Optional[List[float]] = None, anchor_idx: Optional[int] = None) -> list:
         """video -> 4D (pipeline.py:602-685): returns the animated meshes (fixed topology) ordered by timestep."""
-        if stage_0_steps is not None:
-            self.cfg.model.image_to_3D_denoiser.num_inference_steps = stage_0_steps
-        if stage_1_steps is not None:
-            self.scheduler.num_inference_steps = stage_1_steps
-        if guidance_scales is not None:
-            self.cf_guidance.guidance_scales = guidance_scales
-        if face_decimation is not None:
-            self.mesh_process.face_decimation = face_decimation
-        if floaters_threshold is not None:
-            self.mesh_process.floaters_threshold = floaters_threshold
-        if anchor_idx is not None:
-            self.cfg.anchor_idx = anchor_idx
-        if self.background_removal is not None:
-            input.frames = self.background_removal.process_images(input.frames)
-        if self.image_process is not None:
-            input.frames = self.image_process.process_images(input.frames)
-
+        self._apply_overrides(input, stage_0_steps, face_decimation, floaters_threshold, stage_1_steps, guidance_scales,
+                              anchor_idx)
         latent_bank, anchor_mesh = self.init_banks_from_anchor(input, seed)          # Stage 0
         ordered = self._animate(input, latent_bank, anchor_mesh.vertices, anchor_mesh.faces, anchor_mesh.vertex_normals, seed)
         f_np = torch.as_tensor(anchor_mesh.faces).to(torch.int64).numpy()
@@ -469,35 +477,14 @@ class ActionMeshB200PipelineWithMeshInput(ActionMeshB200Pipeline):
         and faces, ordered by timestep."""
         from .mesh_input import denormalize_mesh
 
-        if stage_0_steps is not None:
-            self.cfg.model.image_to_3D_denoiser.num_inference_steps = stage_0_steps
-        if stage_1_steps is not None:
-            self.scheduler.num_inference_steps = stage_1_steps
-        if guidance_scales is not None:
-            self.cf_guidance.guidance_scales = guidance_scales
-        if face_decimation is not None:
-            self.mesh_process.face_decimation = face_decimation
-        if floaters_threshold is not None:
-            self.mesh_process.floaters_threshold = floaters_threshold
-        if anchor_idx is not None:
-            self.cfg.anchor_idx = anchor_idx
-        if self.background_removal is not None:
-            input.frames = self.background_removal.process_images(input.frames)
-        if self.image_process is not None:
-            input.frames = self.image_process.process_images(input.frames)
-
+        self._apply_overrides(input, stage_0_steps, face_decimation, floaters_threshold, stage_1_steps, guidance_scales,
+                              anchor_idx)
         self._load_vae()
         latent_bank, vertex_bank, params, vertex_merge_map, pre_merge_faces = self.init_banks_from_anchor(input, anchor_mesh, seed)
         self._unload_model("vae")
         verts = vertex_bank.get(timesteps=input.timesteps[[self.cfg.anchor_idx]])[0]
         faces = vertex_bank.faces
-        try:
-            import trimesh  # the reference's source of vertex normals (mesh_processor.py:98)
-
-            normals = trimesh.Trimesh(vertices=verts.numpy(), faces=faces.numpy(), process=False).vertex_normals.copy()
-        except ImportError:
-            normals = _vertex_normals(verts, faces)
-        ordered = self._animate(input, latent_bank, verts, faces, normals, seed)
+        ordered = self._animate(input, latent_bank, verts, faces, vertex_normals(verts, faces), seed)
         out = []
         for v in ordered:
             m = denormalize_mesh(Mesh(vertices=v.cpu().numpy().astype(np.float64), faces=None), params)

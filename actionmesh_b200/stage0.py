@@ -25,32 +25,18 @@ import numpy as np
 import torch
 
 from ._lib import AmbError
+from .blocks import remap_triposg_state_dict
 from .denoiser import B200Denoiser, DenoiserConfig
 from .guidance import ClassifierFreeGuidance
 from .scheduler import B200SchedulerFlow
 
-_BLOCK_KEYS = (("norm1.", "norm_s_attn."), ("attn1.", "s_attn."), ("norm2.", "norm_x_attn."), ("attn2.", "x_attn."),
-               ("norm3.", "norm_ff."), ("skip_linear.", "linear_skip."), ("skip_norm.", "norm_skip."))
-
-
-def remap_triposg_state_dict(sd: dict) -> dict:
-    """TripoSGDiTModel keys (DiTBlock norm1/attn1/norm2/attn2/norm3/ff/skip_linear/skip_norm, triposg_transformer.py:190-262)
-    -> the ActionMeshDenoiser keys B200Denoiser packs (block.py:64-108)."""
-    out = {}
-    for k, v in sd.items():
-        if k.startswith("blocks."):
-            _, idx, rest = k.split(".", 2)
-            for a, b in _BLOCK_KEYS:
-                if rest.startswith(a):
-                    rest = b + rest[len(a):]
-                    break
-            k = f"blocks.{idx}.{rest}"
-        out[k] = v
-    return out
-
 
 class B200TripoSGDiT(B200Denoiser):
-    """Drop-in for TripoSGDiTModel on the denoising path: constructor arguments of triposg_transformer.py:412-421."""
+    """Drop-in for TripoSGDiTModel on the denoising path: constructor arguments of triposg_transformer.py:412-421, and
+    `from_pretrained` of a diffusers directory (config.json + diffusion_pytorch_model.safetensors)."""
+
+    config_class = None
+    weight_files = ("diffusion_pytorch_model.safetensors", "diffusion_pytorch_model.bin")
 
     def __init__(self, num_attention_heads: int = 16, width: int = 2048, in_channels: int = 64, num_layers: int = 21,
                  cross_attention_dim: int = 1024, **kwargs):
@@ -60,8 +46,8 @@ class B200TripoSGDiT(B200Denoiser):
                                         num_layers=num_layers, num_attention_heads=num_attention_heads, width=width,
                                         cross_attention_dim=cross_attention_dim, inflated_layers=()))
 
-    def load_state_dict(self, sd: dict) -> None:
-        super().load_state_dict(remap_triposg_state_dict(sd))
+    def _pack_state_dict(self, sd: dict, dev: torch.device) -> dict:
+        return super()._pack_state_dict(remap_triposg_state_dict(sd), dev)
 
     @torch.no_grad()
     def forward(self, hidden_states: torch.Tensor, timestep: torch.Tensor, encoder_hidden_states: torch.Tensor = None,

@@ -19,18 +19,17 @@ rounds the surface to fp16 before embedding it (pipeline_with_3d.py:97-105) and 
 """
 from __future__ import annotations
 
-import json
 import math
-import os
 from dataclasses import dataclass, field
 from typing import Callable, Optional
 
 import numpy as np
 import torch
 
-from . import ops
+from . import blocks, ops
 from ._lib import AmbError
-from .denoiser import repack_cross_kv, repack_self_qkv
+from .blocks import TRIPOSG_BLOCK_KEYS, SyntheticWeights, V, W, pack_block, remap_triposg_state_dict
+from .module import B200Module
 from .pipeline import Mesh, _vertex_normals
 
 DEFAULT_BOUNDS = (-1.005, -1.005, -1.005, 1.005, 1.005, 1.005)   # actionmesh/external/triposg.py:35-100
@@ -200,11 +199,13 @@ def make_mesh(vertices: np.ndarray, faces: np.ndarray):
         return AnchorMesh(vertices=vertices, faces=faces, vertex_normals=n.numpy())
 
 
-class B200TripoSGVAE:
+class B200TripoSGVAE(B200Module):
     """TripoSGVAEModel on the CUDA path: same constructor arguments, state-dict keys (`post_quant.*`, `decoder.*`, and the
     encoder side's `encoder.*`, `quant.*` when present), `from_pretrained(f"{triposg_dir}/vae")`, `decode(z, sampled_points)`
     and, for a user-supplied mesh, `encode(surface)` / `encode_to_latent(surface)` (actionmesh/external/triposg.py:103-172)."""
 
+    config_class = TripoSGVAEConfig
+    weight_files = ("diffusion_pytorch_model.safetensors", "model.safetensors", "diffusion_pytorch_model.bin")
     QUERY_CHUNK = 262144   # query rows per pass: ~4.6 GB of activations at width 1024
 
     def __init__(self, config: Optional[TripoSGVAEConfig] = None, **kwargs):
@@ -218,85 +219,23 @@ class B200TripoSGVAE:
             raise AmbError(f"unsupported width_decoder {c.width_decoder}")
         if c.in_channels != 3:
             raise AmbError("query points must be 3-D")
-        self._device = torch.device("cpu")
-        self._w: dict = {}
-        self._loaded = False
+        super().__init__()
         self._has_encoder = False
         self._qpad = 64 * ((c.query_dim + 63) // 64)
         self._epad = 64 * ((c.encoder_in_dim + 63) // 64)
 
-    # ------------------------------------------------------------------ nn.Module-like surface
-    @property
-    def device(self) -> torch.device:
-        return self._device
-
-    def eval(self):
-        return self
-
-    def to(self, device):
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise AmbError("B200TripoSGVAE only runs on a CUDA (sm_90) device; there is no CPU path")
-        if self._loaded and device != self._device:
-            self._w = {k: v.to(device) for k, v in self._w.items()}
-        self._device = device
-        return self
-
-    @classmethod
-    def from_pretrained(cls, path: str, device="cuda") -> "B200TripoSGVAE":
-        """Diffusers layout: `config.json` + `diffusion_pytorch_model.safetensors` (or `model.safetensors` / `.bin`)."""
-        kwargs = {}
-        cfg_path = os.path.join(path, "config.json")
-        if os.path.exists(cfg_path):
-            raw = json.load(open(cfg_path))
-            kwargs = {k: v for k, v in raw.items() if k in TripoSGVAEConfig.__dataclass_fields__}
-        model = cls(TripoSGVAEConfig(**kwargs)).to(device)
-        for name in ("diffusion_pytorch_model.safetensors", "model.safetensors"):
-            st = os.path.join(path, name)
-            if os.path.exists(st):
-                from safetensors.torch import load_file
-
-                model.load_state_dict(load_file(st))
-                return model
-        model.load_state_dict(torch.load(os.path.join(path, "diffusion_pytorch_model.bin"), map_location="cpu"))
-        return model
-
-    @ops.on_device
-    def load_state_dict(self, sd: dict) -> None:
+    def _pack_state_dict(self, sd: dict, dev: torch.device) -> dict:
         """Pack the weights: bf16 GEMM operands (self-attention QKV fused with the head split folded in, cross K/V likewise,
         proj_query K-padded to 64, proj_out N-padded to 64 and negated); biases and norm weights fp32.  The encoder side
-        (`encoder.*`, `quant.*`: proj_in K-padded 54 -> 64) is packed too when the dict has it."""
+        (`encoder.*`, `quant.*`: proj_in K-padded 54 -> 64) is packed too when the dict has it.  The DiT blocks go through
+        the TripoSG -> ActionMesh key map and are packed under `b{i}.` (decoder) and `e{i}.` (encoder)."""
         c = self.config
-        dev = self._device
-        if dev.type != "cuda":
-            raise AmbError("call .to('cuda') before load_state_dict")
         H, D, L = c.num_attention_heads, c.width_decoder, c.num_layers_decoder
-
-        def f32(name):
-            return sd[name].detach().to(device=dev, dtype=torch.float32).contiguous()
-
-        def W(name):
-            return f32(name).to(torch.bfloat16).contiguous()
-
-        def block(p, q, cross):
-            """DiTBlock `p` (self- or cross-attention, no qk-norm, no qkv bias) -> packed entries under prefix `q`."""
-            norm_attn, attn = ("norm2", "attn2") if cross else ("norm1", "attn1")
-            for src, dst in ((norm_attn, "norm_attn"), ("norm3", "norm_ff")):
-                w[q + dst + ".g"], w[q + dst + ".b"] = f32(p + src + ".weight"), f32(p + src + ".bias")
-            wq, wk, wv = (f32(p + f"{attn}.to_{n}.weight") for n in "qkv")
-            if not cross:
-                w[q + "qkv"] = repack_self_qkv(wq, wk, wv, H).to(torch.bfloat16).contiguous()
-            else:
-                w[q + "q"] = wq.to(torch.bfloat16).contiguous()
-                w[q + "kv"] = repack_cross_kv(wk, wv, H).to(torch.bfloat16).contiguous()
-                w[q + "norm_cross.g"], w[q + "norm_cross.b"] = f32(p + "attn2.norm_cross.weight"), f32(p + "attn2.norm_cross.bias")
-            w[q + "o.w"], w[q + "o.b"] = W(p + f"{attn}.to_out.0.weight"), f32(p + f"{attn}.to_out.0.bias")
-            w[q + "ff1.w"], w[q + "ff1.b"] = W(p + "ff.net.0.proj.weight"), f32(p + "ff.net.0.proj.bias")
-            w[q + "ff2.w"], w[q + "ff2.b"] = W(p + "ff.net.2.weight"), f32(p + "ff.net.2.bias")
-
-        w = {"post_quant.w": W("post_quant.weight"), "post_quant.b": f32("post_quant.bias")}
+        f32 = lambda name: V(sd[name], dev)
+        w = {"post_quant.w": W(sd["post_quant.weight"], dev), "post_quant.b": f32("post_quant.bias")}
+        blk = remap_triposg_state_dict(remap_triposg_state_dict(sd, "decoder.blocks."), "encoder.blocks.")
         for i in range(L + 1):
-            block(f"decoder.blocks.{i}.", f"b{i}.", cross=i == L)
+            pack_block(w, blk, f"decoder.blocks.{i}.", f"b{i}.", H, dev)
         pq = torch.zeros(D, self._qpad, dtype=torch.float32, device=dev)
         pq[:, :c.query_dim].copy_(f32("decoder.proj_query.weight"))
         w["proj_query.w"], w["proj_query.b"] = pq.to(torch.bfloat16), f32("decoder.proj_query.bias")
@@ -314,71 +253,40 @@ class B200TripoSGVAE:
                 raise AmbError(f"B200TripoSGVAE: {why}")
             # block 0 cross-attends from the sampled points to all surface points; blocks 1..L are self-attention
             for i in range(c.num_layers_encoder + 1):
-                block(f"encoder.blocks.{i}.", f"e{i}.", cross=i == 0)
+                pack_block(w, blk, f"encoder.blocks.{i}.", f"e{i}.", H, dev)
             pi = torch.zeros(c.width_encoder, self._epad, dtype=torch.float32, device=dev)
             pi[:, :c.encoder_in_dim].copy_(f32("encoder.proj_in.weight"))
             w["proj_in.w"], w["proj_in.b"] = pi.to(torch.bfloat16), f32("encoder.proj_in.bias")
             w["enc_norm_out.g"], w["enc_norm_out.b"] = f32("encoder.norm_out.weight"), f32("encoder.norm_out.bias")
-            w["quant.w"], w["quant.b"] = W("quant.weight"), f32("quant.bias")
-        self._w = w
-        self._loaded = True
+            w["quant.w"], w["quant.b"] = W(sd["quant.weight"], dev), f32("quant.bias")
+        return w
 
     @ops.on_device
     def init_random_(self, seed: int = 1237) -> None:
         """Synthetic weights for benchmarks (no checkpoints offline), generated on the GPU like B200Autoencoder's."""
         c = self.config
-        dev = self._device
-        g = torch.Generator(device=dev).manual_seed(seed)
         D, L = c.width_decoder, c.num_layers_decoder
-        rs = 1.0 / math.sqrt(L + 1)
-
-        def lin(name, out_f, in_f, scale=1.0, bias=True):
-            bound = 1.0 / math.sqrt(in_f)
-            sd[name + ".weight"] = (torch.rand(out_f, in_f, generator=g, device=dev) * 2 - 1) * bound * scale
-            if bias:
-                sd[name + ".bias"] = (torch.rand(out_f, generator=g, device=dev) * 2 - 1) * bound * scale
-
-        def ln(name, width=None):
-            width = width or D
-            sd[name + ".weight"], sd[name + ".bias"] = torch.ones(width, device=dev), torch.zeros(width, device=dev)
-
-        sd = {}
-        lin("post_quant", D, c.latent_channels)
-        lin("decoder.proj_query", D, c.query_dim)
-        lin("decoder.proj_out", 1, D)
-        ln("decoder.norm_out")
+        sd = SyntheticWeights(seed, self._device)
+        sd.linear("post_quant", D, c.latent_channels)
+        sd.linear("decoder.proj_query", D, c.query_dim)
+        sd.linear("decoder.proj_out", 1, D)
+        sd.layernorm("decoder.norm_out", D)
         for i in range(L + 1):
-            p = f"decoder.blocks.{i}."
-            a = "attn2" if i == L else "attn1"
-            ln(p + ("norm2" if i == L else "norm1"))
-            ln(p + "norm3")
-            if i == L:
-                ln(p + "attn2.norm_cross")
-            for n in ("to_q", "to_k", "to_v"):
-                lin(p + f"{a}.{n}", D, D, bias=False)
-            lin(p + f"{a}.to_out.0", D, D, scale=rs)
-            lin(p + "ff.net.0.proj", 4 * D, D)
-            lin(p + "ff.net.2", D, 4 * D, scale=rs)
+            sd.dit_block(f"decoder.blocks.{i}.", D, 4 * D, 1.0 / math.sqrt(L + 1), ("x_attn" if i == L else "s_attn",),
+                         norm_cross=i == L)
         if c.encoder_supported() is None:
             # encoder from its own generator, so the decoder's weights are the same with or without it
-            g = torch.Generator(device=dev).manual_seed(seed + 1)
             We, Le = c.width_encoder, c.num_layers_encoder
-            rs = 1.0 / math.sqrt(Le + 1)
-            lin("encoder.proj_in", We, c.encoder_in_dim)
-            lin("quant", 2 * c.latent_channels, We)
-            ln("encoder.norm_out", We)
+            enc = SyntheticWeights(seed + 1, self._device)
+            enc.linear("encoder.proj_in", We, c.encoder_in_dim)
+            enc.linear("quant", 2 * c.latent_channels, We)
+            enc.layernorm("encoder.norm_out", We)
             for i in range(Le + 1):
-                p = f"encoder.blocks.{i}."
-                a = "attn2" if i == 0 else "attn1"
-                ln(p + ("norm2" if i == 0 else "norm1"), We)
-                ln(p + "norm3", We)
-                if i == 0:
-                    ln(p + "attn2.norm_cross", We)
-                for n in ("to_q", "to_k", "to_v"):
-                    lin(p + f"{a}.{n}", We, We, bias=False)
-                lin(p + f"{a}.to_out.0", We, We, scale=rs)
-                lin(p + "ff.net.0.proj", 4 * We, We)
-                lin(p + "ff.net.2", We, 4 * We, scale=rs)
+                enc.dit_block(f"encoder.blocks.{i}.", We, 4 * We, 1.0 / math.sqrt(Le + 1), ("x_attn" if i == 0 else "s_attn",),
+                              norm_cross=i == 0)
+            sd.update(enc)
+        to_triposg = [(b, a) for a, b in TRIPOSG_BLOCK_KEYS]
+        sd = blocks.remap_block_keys(blocks.remap_block_keys(sd, to_triposg, "decoder.blocks."), to_triposg, "encoder.blocks.")
         self.load_state_dict(sd)
 
     # ------------------------------------------------------------------ decode
@@ -387,8 +295,7 @@ class B200TripoSGVAE:
     def prepare(self, z: torch.Tensor) -> LatentContext:
         """One latent (N, C) -> the query block's K/V: post_quant, the 16 self-attention blocks (fp32 residual stream), then
         norm_cross and the fused K/V GEMM (autoencoder_kl_triposg.py:199-203,491; attention_processor.py:232-262)."""
-        if not self._loaded:
-            raise AmbError("B200TripoSGVAE: weights not loaded")
+        self._check_loaded()
         c, w, dev = self.config, self._w, self._device
         N = z.shape[0]
         D, H, dh, L = c.width_decoder, c.num_attention_heads, c.head_dim, c.num_layers_decoder
@@ -397,20 +304,12 @@ class B200TripoSGVAE:
         h, xn, qkv, att, ff = E(N, D, dtype=f32), E(N, D), E(N, 3 * D), E(N, D), E(N, 4 * D)
         zb = ops.cast_bf16(z.detach().to(device=dev, dtype=f32).contiguous())
         ops.gemm(zb, w["post_quant.w"], h, bias=w["post_quant.b"], tag="vae_trunk")
-        scale = 1.0 / math.sqrt(dh)
         for i in range(L):
-            q = f"b{i}."
-            ops.layernorm(h, w[q + "norm_attn.g"], w[q + "norm_attn.b"], 1e-5, out=xn)
-            ops.gemm(xn, w[q + "qkv"], qkv, tag="vae_trunk")
-            ops.flash_attn(qkv[:, 0:D].view(1, N, H, dh), qkv[:, D:2 * D].view(1, N, H, dh), qkv[:, 2 * D:].view(1, N, H, dh),
-                           att.view(1, N, H, dh), scale, tag="vae_trunk_attn")
-            ops.gemm(att, w[q + "o.w"], h, bias=w[q + "o.b"], residual=h, tag="vae_trunk")
-            ops.layernorm(h, w[q + "norm_ff.g"], w[q + "norm_ff.b"], 1e-5, out=xn)
-            ops.gemm(xn, w[q + "ff1.w"], ff, bias=w[q + "ff1.b"], act=1, tag="vae_trunk")
-            ops.gemm(ff, w[q + "ff2.w"], h, bias=w[q + "ff2.b"], residual=h, tag="vae_trunk")
+            blocks.attention_half(w, f"b{i}.", h, xn, qkv, att, (1, N), H, tag="vae_trunk", attn_tag="vae_trunk_attn")
+            blocks.output_half(w, f"b{i}.", "s", h, att, xn, ff, tag="vae_trunk")
         q = f"b{L}."
         ops.layernorm(h, w[q + "norm_cross.g"], w[q + "norm_cross.b"], 1e-5, out=xn)
-        kv = ops.gemm(xn, w[q + "kv"], E(N, 2 * D), tag="vae_trunk")          # [K(h,d) | V(h,d)]
+        kv = ops.gemm(xn, w[q + "x.kv"], E(N, 2 * D), tag="vae_trunk")          # [K(h,d) | V(h,d)]
         return LatentContext(kv=kv, k=kv[:, :D].view(1, N, H, dh), v=kv[:, D:].view(1, N, H, dh))
 
     @ops.on_device
@@ -436,14 +335,11 @@ class B200TripoSGVAE:
             e32 = ops.point_embedding(pts[r0:r0 + m], c.embed_frequency, c.embed_include_pi, self._qpad)
             ops.cast_bf16(e32, eb[:m])
             ops.gemm(eb[:m], w["proj_query.w"], x[:m], bias=w["proj_query.b"], tag="vae_query")
-            ops.layernorm(x[:m], w[q + "norm_attn.g"], w[q + "norm_attn.b"], 1e-5, out=xn[:m])
-            ops.gemm(xn[:m], w[q + "q"], qb[:m], tag="vae_query")
+            ops.layernorm(x[:m], w[q + "norm_x_attn.g"], w[q + "norm_x_attn.b"], 1e-5, out=xn[:m])
+            ops.gemm(xn[:m], w[q + "x.q"], qb[:m], tag="vae_query")
             ops.flash_attn(qb[:m].view(1, m, H, dh), ctx.k.view(1, Sk, H, dh), ctx.v.view(1, Sk, H, dh),
                            att[:m].view(1, m, H, dh), scale, tag="vae_query_attn")
-            ops.gemm(att[:m], w[q + "o.w"], x[:m], bias=w[q + "o.b"], residual=x[:m], tag="vae_query")
-            ops.layernorm(x[:m], w[q + "norm_ff.g"], w[q + "norm_ff.b"], 1e-5, out=xn[:m])
-            ops.gemm(xn[:m], w[q + "ff1.w"], ff[:m], bias=w[q + "ff1.b"], act=1, tag="vae_query")
-            ops.gemm(ff[:m], w[q + "ff2.w"], x[:m], bias=w[q + "ff2.b"], residual=x[:m], tag="vae_query")
+            blocks.output_half(w, q, "x", x[:m], att[:m], xn[:m], ff[:m], tag="vae_query")
             ops.layernorm(x[:m], w["norm_out.g"], w["norm_out.b"], 1e-5, out=xn[:m])
             ops.gemm(xn[:m], w["proj_out.w"], out[r0:r0 + m], bias=w["proj_out.b"], tag="vae_query")
         return out
@@ -483,28 +379,20 @@ class B200TripoSGVAE:
         ops.gemm(eq, w["proj_in.w"], h, bias=w["proj_in.b"], tag="vae_encoder")
         ops.gemm(ekv, w["proj_in.w"], ctx, bias=w["proj_in.b"], tag="vae_encoder")
         del ekv, eq
-        scale = 1.0 / math.sqrt(dh)
         # block 0: cross-attention to the norm_cross'ed surface tokens
         q = "e0."
         ops.layernorm(ctx, w[q + "norm_cross.g"], w[q + "norm_cross.b"], 1e-5, out=ctxn)
-        kv = ops.gemm(ctxn, w[q + "kv"], E(N, 2 * D), tag="vae_encoder")          # [K(h,d) | V(h,d)]
+        kv = ops.gemm(ctxn, w[q + "x.kv"], E(N, 2 * D), tag="vae_encoder")          # [K(h,d) | V(h,d)]
         del ctx, ctxn
-        ops.layernorm(h, w[q + "norm_attn.g"], w[q + "norm_attn.b"], 1e-5, out=xn)
-        qb = ops.gemm(xn, w[q + "q"], E(T, D), tag="vae_encoder")
+        ops.layernorm(h, w[q + "norm_x_attn.g"], w[q + "norm_x_attn.b"], 1e-5, out=xn)
+        qb = ops.gemm(xn, w[q + "x.q"], E(T, D), tag="vae_encoder")
         ops.flash_attn(qb.view(1, T, H, dh), kv[:, :D].view(1, N, H, dh), kv[:, D:].view(1, N, H, dh), att.view(1, T, H, dh),
-                       scale, tag="vae_encoder_attn")
+                       1.0 / math.sqrt(dh), tag="vae_encoder_attn")
         del qb, kv
-        for i in range(L + 1):
-            q = f"e{i}."
-            if i > 0:
-                ops.layernorm(h, w[q + "norm_attn.g"], w[q + "norm_attn.b"], 1e-5, out=xn)
-                ops.gemm(xn, w[q + "qkv"], qkv, tag="vae_encoder")
-                ops.flash_attn(qkv[:, 0:D].view(1, T, H, dh), qkv[:, D:2 * D].view(1, T, H, dh),
-                               qkv[:, 2 * D:].view(1, T, H, dh), att.view(1, T, H, dh), scale, tag="vae_encoder_attn")
-            ops.gemm(att, w[q + "o.w"], h, bias=w[q + "o.b"], residual=h, tag="vae_encoder")
-            ops.layernorm(h, w[q + "norm_ff.g"], w[q + "norm_ff.b"], 1e-5, out=xn)
-            ops.gemm(xn, w[q + "ff1.w"], ff, bias=w[q + "ff1.b"], act=1, tag="vae_encoder")
-            ops.gemm(ff, w[q + "ff2.w"], h, bias=w[q + "ff2.b"], residual=h, tag="vae_encoder")
+        blocks.output_half(w, q, "x", h, att, xn, ff, tag="vae_encoder")
+        for i in range(1, L + 1):
+            blocks.attention_half(w, f"e{i}.", h, xn, qkv, att, (1, T), H, tag="vae_encoder", attn_tag="vae_encoder_attn")
+            blocks.output_half(w, f"e{i}.", "s", h, att, xn, ff, tag="vae_encoder")
         ops.layernorm(h, w["enc_norm_out.g"], w["enc_norm_out.b"], 1e-5, out=xn)
         ops.gemm(xn, w["quant.w"], out, bias=w["quant.b"], tag="vae_encoder")
         return out
@@ -530,6 +418,7 @@ class B200TripoSGVAE:
         idx = ops.farthest_point_sample(selected, num_tokens, start)
         return selected[torch.arange(B, device=x.device)[:, None], idx], idx
 
+    @ops.on_device
     @torch.no_grad()
     def encode(self, x: torch.Tensor, return_dict: bool = True, num_tokens: int = 2048, seed: Optional[int] = None,
                generator: Optional[torch.Generator] = None):
@@ -537,12 +426,11 @@ class B200TripoSGVAE:
         (B, N, 6) surface [xyz | normal] -> `.latent_dist`, a `DiagonalGaussianDistribution` of (B, num_tokens, C).
         `seed` fixes the host subset, `generator` the FPS start (and is the natural one to pass to `.sample`)."""
         x = x.detach().to(device=self._device, dtype=torch.float32).contiguous()
-        with torch.cuda.device(self._device):
-            sampled, _ = self.sample_features(x, num_tokens, seed, generator)
-            params = torch.empty(x.shape[0], num_tokens, 2 * self.config.latent_channels, dtype=torch.float32, device=self._device)
-            for b in range(x.shape[0]):
-                self.encode_points(x[b], sampled[b], out=params[b])
-            posterior = DiagonalGaussianDistribution(params)
+        sampled, _ = self.sample_features(x, num_tokens, seed, generator)
+        params = torch.empty(x.shape[0], num_tokens, 2 * self.config.latent_channels, dtype=torch.float32, device=self._device)
+        for b in range(x.shape[0]):
+            self.encode_points(x[b], sampled[b], out=params[b])
+        posterior = DiagonalGaussianDistribution(params)
         return EncoderOutput(latent_dist=posterior) if return_dict else (posterior,)
 
     @torch.no_grad()
@@ -553,6 +441,7 @@ class B200TripoSGVAE:
         return self.encode(surface, seed=seed, generator=generator).latent_dist.sample(generator)
 
     # ------------------------------------------------------------------ mesh
+    @ops.on_device
     @torch.no_grad()
     def extract_geometry(self, latents: torch.Tensor, bounds=DEFAULT_BOUNDS, octree_depth: int = 9,
                          decode: Optional[Callable] = None) -> list:
@@ -565,9 +454,8 @@ class B200TripoSGVAE:
                 fn = lambda xyz, ctx=ctx: self.query(ctx, xyz)
             else:
                 fn = decode
-            with torch.cuda.device(self._device):
-                grid = refine_octree(fn, bounds, octree_depth, self._device)
-                out.append(mesh_from_grid(grid, bounds, octree_depth))
+            grid = refine_octree(fn, bounds, octree_depth, self._device)
+            out.append(mesh_from_grid(grid, bounds, octree_depth))
             del grid
         return out
 

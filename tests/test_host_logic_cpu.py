@@ -4,7 +4,7 @@ import torch
 import os
 
 from conftest import ROOT, load_golden
-from actionmesh_b200.denoiser import repack_cross_kv, repack_self_qkv
+from actionmesh_b200.blocks import repack_cross_kv, repack_self_qkv
 from actionmesh_b200.guidance import ClassifierFreeGuidance
 from actionmesh_b200.scheduler import B200SchedulerFlow
 

@@ -1,12 +1,16 @@
-"""Structural CPU test of the denoiser's launch programs (no GPU, no arithmetic): `B200Denoiser._forward_packed` (single
-GPU) and the staggered per-branch programs of the frame-sharded window are executed against shape/dtype-checking fakes of
-the C-ABI wrappers in actionmesh_b200.ops.  Catches slicing / buffer-plumbing / generator-flow mistakes in the host code
+"""Structural CPU test of the host launch programs (no GPU, no arithmetic): `B200Denoiser._forward_packed` (single GPU) and
+the staggered per-branch programs of the frame-sharded window, `B200Autoencoder.forward`, `B200TripoSGVAE.prepare` / `query`
+/ `encode_points` and `B200ImageEncoder.encode_pixel_values` are executed against shape/dtype-checking fakes of the C-ABI
+wrappers in actionmesh_b200.ops, with weights packed on the CPU.  Catches slicing / buffer-plumbing / generator-flow mistakes in the host code
 that would otherwise only show on a GPU box; the numerics are covered by the -m gpu parity tests."""
 import pytest
 import torch
 
 from actionmesh_b200 import denoiser as dn
 from actionmesh_b200 import ops
+from actionmesh_b200.autoencoder import AutoencoderConfig, B200Autoencoder
+from actionmesh_b200.image_encoder import B200ImageEncoder
+from actionmesh_b200.triposg_vae import B200TripoSGVAE
 from oracle import synth
 
 
@@ -68,11 +72,63 @@ class _Recorder:
         self.calls.append(("cast", tuple(src.shape)))
         return out
 
+    def split3(self, src, out, seg=None, weight=False):
+        rows, cols = src.shape
+        assert src.dtype == torch.float32 and out.dtype == torch.bfloat16 and out.shape[0] >= rows and out.shape[1] == 3 * cols
+        assert cols % (seg or cols) == 0
+        self.calls.append(("split3", tuple(src.shape)))
+        return out
+
+    def point_embedding(self, points, num_freqs, include_pi, kpad):
+        assert points.dtype == torch.float32 and points.dim() == 2
+        assert kpad % 64 == 0 and kpad >= 3 * (2 * num_freqs + 1) + points.shape[1] - 3
+        return torch.empty(points.shape[0], kpad, dtype=torch.float32)
+
+    def alpha_rows(self, source_alpha, target_alpha, size, out_rows):
+        assert out_rows.dtype == torch.float32 and out_rows.dim() == 2 and out_rows.shape[1] == 2 * size
+        self.calls.append(("alpha_rows", tuple(out_rows.shape)))
+
+    def softmax_split3(self, scores, n, scale, out):
+        rows, n_pad = scores.shape
+        assert scores.dtype == torch.float32 and n <= n_pad and out.shape == (rows, 3 * n_pad)
+        self.calls.append(("softmax_split3", tuple(scores.shape)))
+        return out
+
+    def displacement_out(self, logits, out_dim, out):
+        assert logits.dtype == out.dtype == torch.float32 and out.numel() == logits.shape[0] * out_dim
+        self.calls.append(("displacement_out", tuple(out.shape)))
+        return out
+
+    def attn_small_f32(self, qkv, frames, seq, heads, scale, out, tag="attn_small"):
+        assert qkv.dtype == out.dtype == torch.float32
+        assert qkv.shape == (frames * seq, 3 * heads * 64) and out.shape == (frames * seq, heads * 64)
+        self.calls.append((tag, (frames, seq, heads, 64), (frames, seq, heads, 64)))
+        return out
+
+    def patchify(self, pixels, patch, kpad, out=None):
+        T, C, H, W = pixels.shape
+        assert C == 3 and pixels.dtype == torch.float32 and kpad >= 3 * patch * patch
+        return torch.empty(T * (H // patch) * (W // patch), kpad, dtype=torch.bfloat16)
+
+
+def _recorder(monkeypatch):
+    rec = _Recorder()
+    for name in ("gemm", "layernorm", "flash_attn", "timestep_embedding", "add_bias_rows", "cast_bf16", "split3",
+                 "point_embedding", "alpha_rows", "softmax_split3", "displacement_out", "attn_small_f32", "patchify"):
+        monkeypatch.setattr(ops, name, getattr(rec, name))
+    return rec
+
+
+def _load_on_cpu(m):
+    """init_random_'s weights, packed on the CPU (load_state_dict needs a CUDA device)."""
+    m.load_state_dict = lambda sd: setattr(m, "_w", m._pack_state_dict(sd, torch.device("cpu")))
+    m.init_random_()
+    m._loaded = True
+    return m
+
 
 def _model(monkeypatch, residual_fp32=True):
-    rec = _Recorder()
-    for name in ("gemm", "layernorm", "flash_attn", "timestep_embedding", "add_bias_rows", "cast_bf16"):
-        monkeypatch.setattr(ops, name, getattr(rec, name))
+    rec = _recorder(monkeypatch)
     d = dict(num_layers=5, num_attention_heads=2, width=256, cross_attention_dim=128, in_channels=64, mlp_ratio=4.0)
     cfg = dn.DenoiserConfig(inflated_layers=(0, 1, 2, 3, 4), **d)
     m = dn.B200Denoiser(cfg, residual_fp32=residual_fp32)
@@ -144,3 +200,46 @@ def test_sharded_branch_programs_interleave(monkeypatch):
             assert not (tags[i + 1][0] == "wait" and tags[i + 1][1] == tags[i][1]), "a gather was waited on immediately"
     attn = [c for c in rec.calls if c[0] == "attn_self"]
     assert len(attn) == B * cfg.num_layers and all(c[1] == (1, T * (N + 1), 2, 128) and c[2][:3] == (1, world, T * (N + 1)) for c in attn)
+
+
+def test_autoencoder_program(monkeypatch):
+    rec = _recorder(monkeypatch)
+    cfg = AutoencoderConfig(width=256, num_layers=2, num_attention_heads=2, temporal_context_size=4)
+    m = _load_on_cpu(B200Autoencoder(cfg))
+    B, T, N, V, T_out = 2, 4, 15, 20, 3
+    out = m.forward(torch.randn(B, T, N, 64), torch.arange(T, dtype=torch.float32)[None].repeat(B, 1) + 3,
+                    torch.full((B,), 0.25), torch.rand(B, T_out), torch.randn(B, V, 6))
+    assert out.shape == (B, T_out, V, 3) and out.dtype == torch.float32
+    trunk = [c for c in rec.calls if c[0] == "s2_attn"]
+    assert len(trunk) == B * T_out * cfg.num_layers and all(c[1] == (1, T * (N + 1), 2, 128) for c in trunk)
+    assert sum(1 for c in rec.calls if c[0] == "softmax_split3") == B * T_out * cfg.num_attention_heads
+    assert sum(1 for c in rec.calls if c[0] == "alpha_rows") == B * T_out
+    assert sum(1 for c in rec.calls if c[0] == "displacement_out") == B * T_out
+
+
+def test_triposg_vae_programs(monkeypatch):
+    rec = _recorder(monkeypatch)
+    m = _load_on_cpu(B200TripoSGVAE(width_decoder=256, num_attention_heads=2, num_layers_decoder=2, width_encoder=256,
+                                    num_layers_encoder=2))
+    assert m._has_encoder
+    N, P, chunk = 33, 50, 20
+    ctx = m.prepare(torch.randn(N, 64))
+    assert ctx.kv.shape == (N, 2 * 256) and ctx.k.shape == ctx.v.shape == (1, N, 2, 128)
+    assert [c[1] for c in rec.calls if c[0] == "vae_trunk_attn"] == [(1, N, 2, 128)] * 2
+    assert m.query(ctx, torch.randn(P, 3), chunk=chunk).shape == (P, 64)
+    assert [c[1:] for c in rec.calls if c[0] == "vae_query_attn"] == [((1, m_, 2, 128), (1, N, 2, 128)) for m_ in (20, 20, 10)]
+    n_kv, n_q = 40, 16
+    assert m.encode_points(torch.randn(n_kv, 6), torch.randn(n_q, 6)).shape == (n_q, 2 * 64)
+    enc = [c[1:] for c in rec.calls if c[0] == "vae_encoder_attn"]
+    assert enc == [((1, n_q, 2, 128), (1, n_kv, 2, 128))] + [((1, n_q, 2, 128), (1, n_q, 2, 128))] * 2
+
+
+@pytest.mark.parametrize("precision", ["fp32", "bf16"])
+def test_image_encoder_program(monkeypatch, precision):
+    rec = _recorder(monkeypatch)
+    m = _load_on_cpu(B200ImageEncoder(hidden_size=256, num_layers=2, num_heads=4, image_size=28, precision=precision))
+    T, L = 3, 1 + 2 * 2
+    out = m.encode_pixel_values(torch.randn(T, 3, 28, 28))
+    assert out.shape == (T, L, 256) and out.dtype == torch.float32
+    attn = [c[1] for c in rec.calls if c[0] == "attn_dino"]
+    assert attn == [(T, L, 4, 64)] * 2
