@@ -106,14 +106,30 @@ def group_elementwise(res):
     res["add_bias_rows"] = _err(y, r)
 
 
+def _gemm_kernel(fn):
+    """Name of the GEMM kernel one call of fn launches (gemm_bf16_kernel<BN>), read from a torch.profiler trace."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    names = set()
+    for _ in range(3):  # a short trace now and then comes back without its kernel record
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        names = {e.name for e in prof.events() if "gemm_bf16_kernel" in e.name}
+        if names:
+            break
+    return ",".join(sorted(n[n.index("gemm_bf16_kernel"):].split("(")[0] for n in names))
+
+
 def _gemm_case(res, name, m, n, k, *, bias=False, act=0, residual=False, a2=False, row_map=None, out_fp32=False,
-               res_fp32=False, col_scale=False, norm=None, timing=False, seed=1):
+               res_fp32=False, col_scale=False, norm=None, timing=False, seed=1, alias=False, out2=False):
     import torch
     from actionmesh_b200 import ops
     dev = "cuda"
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    A = (torch.randn(m, k, generator=g) * 0.5).to(dev).bfloat16()
-    W = (torch.randn(n, k, generator=g) / math.sqrt(k)).to(dev).bfloat16()
+    g = torch.Generator(device=dev).manual_seed(seed)
+    A = (torch.randn(m, k, generator=g, device=dev) * 0.5).bfloat16()
+    W = (torch.randn(n, k, generator=g, device=dev) / math.sqrt(k)).bfloat16()
     kw = {}
     ref = A.float() @ W.float().t()
     if a2:
@@ -126,11 +142,11 @@ def _gemm_case(res, name, m, n, k, *, bias=False, act=0, residual=False, a2=Fals
         Ain = A
     if norm is not None:
         nc, seg, rc, rpp = norm
-        w0 = (torch.rand(128, generator=g) + 0.5).to(dev)
-        w1 = (torch.rand(128, generator=g) + 0.5).to(dev)
+        w0 = torch.rand(128, generator=g, device=dev) + 0.5
+        w1 = torch.rand(128, generator=g, device=dev) + 0.5
         npos = (m + rpp - 1) // rpp
-        ang = torch.rand(npos, 64, generator=g) * 6.28
-        cos, sin = ang.cos().to(dev), ang.sin().to(dev)
+        ang = torch.rand(npos, 64, generator=g, device=dev) * 6.28
+        cos, sin = ang.cos(), ang.sin()
         kw["norm"] = dict(cols=nc, seg=seg, w0=w0, w1=w1, eps=1e-6, rope_cols=rc, cos=cos, sin=sin, rows_per_pos=rpp)
         r = ref.clone()
         for c0 in range(0, nc, 128):
@@ -146,7 +162,7 @@ def _gemm_case(res, name, m, n, k, *, bias=False, act=0, residual=False, a2=Fals
             r[:, c0:c0 + 128] = h
         ref = r
     if bias:
-        bv = torch.randn(n, generator=g).to(dev)
+        bv = torch.randn(n, generator=g, device=dev)
         kw["bias"] = bv
         if norm is None:
             ref = ref + bv
@@ -156,7 +172,7 @@ def _gemm_case(res, name, m, n, k, *, bias=False, act=0, residual=False, a2=Fals
         kw["act"] = 1
         ref = torch.nn.functional.gelu(ref)
     if col_scale:
-        cs = torch.randn(n, generator=g).to(dev)
+        cs = torch.randn(n, generator=g, device=dev)
         kw["col_scale"] = cs
         ref = ref * cs
     mo = m
@@ -166,9 +182,15 @@ def _gemm_case(res, name, m, n, k, *, bias=False, act=0, residual=False, a2=Fals
         kw["row_map"] = row_map
     out = torch.full((mo, n), 7.0, device=dev, dtype=torch.float32 if out_fp32 else torch.bfloat16)
     if residual:
-        R = torch.randn(mo, n, generator=g).to(dev)
+        R = torch.randn(mo, n, generator=g, device=dev)
         R = R if res_fp32 else R.bfloat16()
-        kw["residual"] = R
+        if alias:  # the residual stream updated in place, as the denoiser runs it
+            out.copy_(R)
+            kw["residual"] = out
+        else:
+            kw["residual"] = R
+    if out2:
+        kw["out2"] = torch.empty(mo, n, device=dev, dtype=torch.bfloat16)
     ops.gemm(Ain, W, out, **kw)
     torch.cuda.synchronize()
     if row_map is not None:
@@ -177,17 +199,18 @@ def _gemm_case(res, name, m, n, k, *, bias=False, act=0, residual=False, a2=Fals
         drow = (rows // gr) * gs + rows % gr + ro
         full = torch.full((mo, n), 7.0, device=dev)
         if residual:
-            full[drow] = ref + kw["residual"].float()[drow]
+            full[drow] = ref + R.float()[drow]
         else:
             full[drow] = ref
         ref = full
     elif residual:
-        ref = ref + kw["residual"].float()
+        ref = ref + R.float()
     res[name] = _err(out, ref)
     if timing:
-        ms = _time(lambda: ops.gemm(Ain, W, out, **kw), iters=5)
+        ms = _time(lambda: ops.gemm(Ain, W, out, **kw), iters=20)
         res[name]["ms"] = ms
         res[name]["TFLOPs"] = 2.0 * m * n * k / ms / 1e9
+        res[name]["kernel"] = _gemm_kernel(lambda: ops.gemm(Ain, W, out, **kw))
 
 
 def group_gemm(res):
@@ -215,14 +238,24 @@ def _cublas_case(res, m, n, k):
 
 
 def group_gemm_perf(res):
+    res["card"] = _card()
     _gemm_case(res, "p_8192x2048x2048", 8192, 2048, 2048, timing=True)
     _gemm_case(res, "p_65568x2048x2048_res", 65568, 2048, 2048, bias=True, residual=True, timing=True)
     _gemm_case(res, "p_65568x8192x2048_gelu", 65568, 8192, 2048, bias=True, act=1, timing=True)
     _gemm_case(res, "p_65568x2048x8192_res", 65568, 2048, 8192, bias=True, residual=True, timing=True)
     _gemm_case(res, "p_65568x6144x2048_qkv", 65568, 6144, 2048, norm=(4096, 2048, 4096, 2049), timing=True)
     _gemm_case(res, "p_65568x2048x4096_skip", 65568, 2048, 4096, a2=True, bias=True, timing=True)
+    # the block GEMMs with the epilogues the fp32-stream denoiser launches: s.o and x.o update the fp32 residual stream in
+    # place, ff2 also writes its bf16 copy; x.q (q-norm) and x.o run once per CFG branch with image context (M = 16 x 2049)
+    _gemm_case(res, "p_65568x2048x2048_s.o_f32", 65568, 2048, 2048, bias=True, residual=True, res_fp32=True, out_fp32=True,
+               alias=True, timing=True)
+    _gemm_case(res, "p_65568x2048x8192_ff2_f32", 65568, 2048, 8192, bias=True, residual=True, res_fp32=True, out_fp32=True,
+               alias=True, out2=True, timing=True)
+    _gemm_case(res, "p_32784x2048x2048_x.q", 32784, 2048, 2048, norm=(2048, 2048, 0, 1), timing=True)
+    _gemm_case(res, "p_32784x2048x2048_x.o_f32", 32784, 2048, 2048, bias=True, residual=True, res_fp32=True, out_fp32=True,
+               alias=True, timing=True)
     for m, n, k in ((8192, 2048, 2048), (65568, 2048, 2048), (65568, 8192, 2048), (65568, 2048, 8192),
-                    (65568, 6144, 2048), (65568, 2048, 4096)):
+                    (65568, 6144, 2048), (65568, 2048, 4096), (32784, 2048, 2048)):
         _cublas_case(res, m, n, k)
 
 
