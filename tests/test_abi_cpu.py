@@ -1,8 +1,10 @@
-"""C-ABI checks that need no GPU: the library loads, exports every symbol include/actionmesh_b200.h declares, and
-argument validation fails loudly with an error code + message (no compute calls)."""
+"""C-ABI checks that need no GPU: the library loads, exports every symbol include/actionmesh_b200.h declares, the
+ctypes binding read from that header has its signatures and struct layouts, and argument validation fails loudly with
+an error code + message (no compute calls)."""
 import ctypes as C
 import os
 import re
+import subprocess
 
 import pytest
 
@@ -35,31 +37,57 @@ def test_binding_matches_header(amb_lib):
     assert amb_lib.amb_abi_version() == ver == _lib.ABI_VERSION
 
 
-def test_struct_layouts_match_header(amb_lib):
-    """ctypes struct sizes equal the C structs' (computed from the header field order with natural alignment)."""
+def test_struct_layouts_match_header(tmp_path):
+    """Every field offset and the size of the ctypes structs equal the C compiler's offsetof / sizeof for the header."""
     from actionmesh_b200 import _lib
 
-    text = open(os.path.join(ROOT, "include", "actionmesh_b200.h")).read()
+    structs = (("amb_gemm_args", _lib.GemmArgs), ("amb_attn_args", _lib.AttnArgs))
+    prints = [f'printf("%zu\\n", sizeof({cname}));' for cname, _ in structs]
+    prints += [f'printf("%zu\\n", offsetof({cname}, {f}));' for cname, cls in structs for f, _ in cls._fields_]
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "actionmesh_b200.h"\nint main(void) {\n'
+                   + "\n".join(prints) + "\nreturn 0;\n}\n")
+    exe = tmp_path / "layout"
+    subprocess.run(["cc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
+    got = [int(v) for v in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
+    want = [C.sizeof(cls) for _, cls in structs] + [getattr(cls, f).offset for _, cls in structs for f, _ in cls._fields_]
+    assert got == want
 
-    def csize(struct_name):
-        body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (struct_name, struct_name), text, flags=re.S).group(1)
-        body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-        off = 0
-        for decl in body.split(";"):
-            decl = decl.strip()
-            if not decl:
-                continue
-            m = re.match(r"(const\s+)?(void|float|int64_t|int32_t)\s*(\*)?\s*(.*)", decl)
-            assert m, decl
-            base, ptr, names = m.group(2), m.group(3), m.group(4)
-            for nm in names.split(","):
-                is_ptr = bool(ptr) or nm.strip().startswith("*")
-                sz = 8 if (is_ptr or base == "int64_t") else 4
-                off = (off + sz - 1) // sz * sz + sz
-        return (off + 7) // 8 * 8
 
-    assert C.sizeof(_lib.GemmArgs) == csize("amb_gemm_args")
-    assert C.sizeof(_lib.AttnArgs) == csize("amb_attn_args")
+def test_binding_maps_every_parameter(amb_lib):
+    """The header parse binds every declared function with one ctypes type per declared parameter, and load_library
+    applies exactly those types."""
+    from actionmesh_b200 import _lib
+
+    prototypes, _ = _lib.parse_header(_lib.HEADER_PATH)
+    assert sorted(prototypes) == _declared_functions()
+    text = re.sub(r"/\*.*?\*/", "", open(_lib.HEADER_PATH).read(), flags=re.S)
+    for name, (restype, argtypes) in prototypes.items():
+        params = re.search(r"\b%s\s*\(([^)]*)\)" % name, text).group(1).strip()
+        assert len(argtypes) == (0 if params == "void" else params.count(",") + 1), name
+        fn = getattr(amb_lib, name)
+        assert tuple(fn.argtypes) == tuple(argtypes) and fn.restype is restype, name
+    P = C.c_void_p
+    assert prototypes["amb_cfg_euler_step"] == (C.c_int, [P, P, C.c_int, P, C.c_float, P, C.c_int, C.c_int64, C.c_int64,
+                                                          C.c_int64, C.c_int64, P])
+    assert prototypes["amb_mesh_collapse_apply"][1][6] is C.c_uint64
+    assert prototypes["amb_last_error"] == (C.c_char_p, [])
+
+
+@pytest.mark.parametrize("decl", [
+    "int amb_bad(const float* x, double scale, amb_stream_t stream);",      # unknown scalar
+    "int amb_bad(const size_t* x, amb_stream_t stream);",                  # unknown pointee
+    "int amb_bad(const float** x, amb_stream_t stream);",                  # pointer to pointer
+    "void amb_bad(int n);",                                                # unknown return type
+    "typedef struct amb_bad_args { int32_t m; long n; } amb_bad_args;",    # unknown member type
+])
+def test_header_parse_refuses_unknown_types(tmp_path, decl):
+    from actionmesh_b200 import _lib
+
+    header = tmp_path / "bad.h"
+    header.write_text("/* comment */\nint amb_ok(int n, amb_stream_t stream);\n" + decl + "\n")
+    with pytest.raises(_lib.AmbError, match="amb_bad"):
+        _lib.parse_header(str(header))
 
 
 def test_argument_validation_fails_loudly(amb_lib):
