@@ -466,6 +466,9 @@ int amb_split3_bf16(const float* src, int64_t ld_src, int64_t rows, int cols, in
   AMB_CHECK_ARG(cols > 0 && seg > 0 && cols % seg == 0 && seg % 4 == 0 && ld_src % 4 == 0 && ld_dst % 4 == 0 &&
                     ld_dst >= 3LL * cols && ld_src >= cols,
                 "split3: bad geometry cols=%d seg=%d ld_src=%lld ld_dst=%lld", cols, seg, (long long)ld_src, (long long)ld_dst);
+  // the kernel reads float4 and writes 4-element bf16 vectors (uint2)
+  AMB_CHECK_ARG((reinterpret_cast<uintptr_t>(src) & 15) == 0, "split3: src must be 16-byte aligned");
+  AMB_CHECK_ARG((reinterpret_cast<uintptr_t>(dst_bf16) & 7) == 0, "split3: dst must be 8-byte aligned");
   if (rows <= 0) return AMB_OK;
   split3_kernel<<<grid_for(rows * (cols / 4), 256), 256, 0, (cudaStream_t)stream>>>(
       src, ld_src, rows, cols, seg, w_pattern, reinterpret_cast<__nv_bfloat16*>(dst_bf16), ld_dst);
@@ -478,6 +481,8 @@ int amb_softmax_split3(const float* scores, int64_t ld_s, int rows, int n, int n
   AMB_CHECK_ARG(scores && dst_bf16, "softmax_split3: null pointer");
   AMB_CHECK_ARG(n > 0 && n_pad >= n && n_pad % 4 == 0 && ld_s % 4 == 0 && ld_s >= n_pad && ld_dst % 4 == 0 && ld_dst >= 3LL * n_pad,
                 "softmax_split3: bad geometry n=%d n_pad=%d", n, n_pad);
+  AMB_CHECK_ARG((reinterpret_cast<uintptr_t>(scores) & 15) == 0, "softmax_split3: scores must be 16-byte aligned");
+  AMB_CHECK_ARG((reinterpret_cast<uintptr_t>(dst_bf16) & 7) == 0, "softmax_split3: dst must be 8-byte aligned");
   if (rows <= 0) return AMB_OK;
   softmax_split3_kernel<<<rows, 512, 0, (cudaStream_t)stream>>>(scores, ld_s, n, n_pad, scale,
                                                                   reinterpret_cast<__nv_bfloat16*>(dst_bf16), ld_dst);

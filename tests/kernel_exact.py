@@ -193,6 +193,8 @@ GEMM_CONFIGS = [
     GemmConfig("bn64_n192_res_f32", 192, 128, out="f32", bias=True, residual="alias", res="f32"),
     GemmConfig("bn64_n320_res_f32", 320, 128, out="f32", bias=True, residual="alias", res="f32"),
     GemmConfig("bn64_n320_res_bf16", 320, 128, bias=True, residual="alias"),
+    # Stage II's score GEMM S = Q'K'^T and V-transpose GEMM V^T = W_v ctx^T: fp32, no bias, N = Rp = 64 mod 128
+    GemmConfig("bn64_n192_f32", 192, 128, out="f32"),
 ]
 GEMM_CONFIG = {c.name: c for c in GEMM_CONFIGS}
 

@@ -156,4 +156,27 @@ def test_argument_validation_of_widened_entry_points(amb_lib):
     assert amb_lib.amb_resize_v_normalize(P, 1, 8, 0, 32, P, P, 9, 32, None, m, m, P, None, None) < 0 and "null pointer" in err()
     # zero-size work is a successful no-op without a launch
     assert amb_lib.amb_split3_bf16(P, 128, 0, 128, 128, 0, P, 384, None) == 0
+    assert amb_lib.amb_softmax_split3(P, 128, 0, 100, 128, 1.0, P, 384, None) == 0
     assert amb_lib.amb_resize_h_u8(P, 0, 64, 64, 3, 0, 64, P, P, 9, 32, P, None) == 0
+
+
+@pytest.mark.parametrize("src,dst", [(16 + 4, 16), (16 + 8, 16), (16, 16 + 2), (16, 16 + 4), (16 + 4, 16 + 2)])
+def test_split_operands_refuse_misaligned_pointers(amb_lib, src, dst):
+    """split3 reads float4 and writes 4-element bf16 vectors, softmax_split3 the same: a source that is not 16-byte
+    aligned or a destination that is not 8-byte aligned (a column-offset view such as x[:, 1:]) is refused before any
+    launch, naming the argument; zero rows do not skip the check (fake non-null pointers)."""
+    err = lambda: amb_lib.amb_last_error().decode()
+    name = "src" if src % 16 else "dst"
+    for rows in (1, 0):
+        assert amb_lib.amb_split3_bf16(src, 128, rows, 128, 128, 0, dst, 384, None) < 0
+        assert f"split3: {name} must be" in err()
+        assert amb_lib.amb_softmax_split3(src, 128, rows, 100, 128, 1.0, dst, 384, None) < 0
+        assert f"softmax_split3: {'scores' if name == 'src' else 'dst'} must be" in err()
+
+
+def test_split_operands_accept_aligned_pointers(amb_lib):
+    """The smallest alignments the kernels need pass validation: 16-byte sources, 8-byte destinations (zero rows: no
+    launch)."""
+    assert amb_lib.amb_split3_bf16(32, 128, 0, 128, 128, 0, 24, 384, None) == 0
+    assert amb_lib.amb_softmax_split3(32, 128, 0, 100, 128, 1.0, 24, 384, None) == 0
+    assert amb_lib.amb_split3_bf16(16, 128, 0, 128, 128, 0, 8, 384, None) == 0
