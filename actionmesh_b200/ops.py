@@ -413,11 +413,12 @@ def octree_dilate(mask: torch.Tensor, out: Optional[torch.Tensor] = None) -> tor
     return out
 
 
-def octree_mark_upsampled(mask: torch.Tensor) -> torch.Tensor:
-    """(n,n,n) uint8 -> (2n-1)^3 uint8 with fine[2x, 2y, 2z] = mask[x, y, z] and zeros elsewhere."""
+def octree_mark_upsampled(mask: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """(n,n,n) uint8 -> (2n-1)^3 uint8 with fine[2x, 2y, 2z] = (mask[x, y, z] != 0) and zeros elsewhere."""
     dev = _device(mask, "mask")
     n = _cube(mask, "mask")
-    fine = torch.empty((2 * n - 1,) * 3, dtype=torch.uint8, device=mask.device)
+    fine = torch.empty((2 * n - 1,) * 3, dtype=torch.uint8, device=mask.device) if out is None else out
+    assert _cube(fine, "out") == 2 * n - 1, "out: expected a (2n-1)^3 cube"
     _launch(_abi.amb_octree_mark_upsampled, 2, _ptr(mask, torch.uint8, "mask", dev), n, _ptr(fine, torch.uint8, "fine", dev))
     return fine
 

@@ -1,5 +1,7 @@
 """Stage 0's anchor-mesh path without a GPU: the fp32 decode restatement against the reference's own TripoSG VAE, the numpy
-dual-marching-cubes restatement on analytic surfaces, the committed patch table and the octree resolution ladder."""
+dual-marching-cubes restatement on analytic surfaces, the committed patch table (also against an independent derivation),
+the octree resolution ladder and the grid sides the geometry tests run, and the torch restatement of the near-surface band
+against the reference's own band."""
 import math
 import os
 import subprocess
@@ -9,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+import geometry_exact as gx
 import triposg_vae_ref as ref
 from conftest import ROOT, load_golden
 
@@ -67,6 +70,46 @@ def test_patch_table_properties():
         assert all(len(np.nonzero(pe[case] == p)[0]) >= 3 for p in range(npatch[case]))   # a patch has >= 3 crossings
     # two inside corners on a face diagonal stay separated (corners 0 and 3 of the z = 0 face)
     assert npatch[0b00001001] == 2
+
+
+def test_patch_table_header_matches_independent_derivation():
+    """csrc/dmc_table.cuh, read as text, equals the table derived from corner components (geometry_exact)."""
+    pe, cnt = gx.header_tables()
+    ipe, icnt = gx.independent_tables()
+    assert np.array_equal(pe, ipe) and np.array_equal(cnt, icnt)
+    assert np.bincount(cnt).tolist() == [2, 162, 82, 8, 2]
+
+
+def test_dyadic_expectation_matches_restatement():
+    """On a dyadic grid the vertex bits from the independent table equal dmc_numpy's, and its mesh has the table-free
+    invariants the GPU tests assert."""
+    g = gx.dyadic_grid(24, 5, outside_border=True)
+    exp = gx.dmc_expected(g)
+    v, f = ref.dmc_numpy(g)
+    assert np.array_equal(exp["vertices"].view(np.int32), v.view(np.int32))
+    assert len(f) == gx.expected_face_count(g) > 0 and gx.faces_nondegenerate(f) and gx.directed_edges_paired(f)
+    assert gx.vertices_in_cells(v, exp["cell_of_vertex"], 23) and gx.signed_volume(v, f) > 0
+
+
+def test_geometry_sides_cover_the_depth9_ladder():
+    """Every grid the depth-9 refinement launches a geometry kernel on is a side the exact tests run: each level's grid
+    n = r + 1 and each fine mask 2n - 1 that mark_upsampled writes."""
+    from actionmesh_b200.triposg_vae import octree_resolutions
+
+    sides = [r + 1 for r in octree_resolutions(9)]
+    fine = [2 * n - 1 for n in sides[:-1]]
+    assert set(sides) | set(fine) <= set(gx.SIDES), sorted((set(sides) | set(fine)) - set(gx.SIDES))
+    assert fine[-1] == sides[-1] == max(gx.SIDES) and max(gx.SCAN_SIDES) == sides[-1]
+
+
+@pytest.mark.parametrize("n", [2, 3, 12, 13, 16])
+def test_band_restatement_matches_reference(n):
+    """geometry_exact.near_surface_ref equals the reference's extract_near_surface_volume_fn + |v| < 0.95 (golden) on the
+    adversarial band grids."""
+    gold = load_golden("octree_fields.pt")["bands"][n]
+    g = gx.band_grid(n)
+    assert ref.sha256(g) == gold["sha256_grid"]
+    assert torch.equal(gx.near_surface_ref(g), gold["mask"])
 
 
 def test_octree_resolution_ladder():
