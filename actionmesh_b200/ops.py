@@ -671,3 +671,74 @@ def mesh_face_components(edges: torch.Tensor, n_faces: int) -> tuple[torch.Tenso
     sizes = torch.empty_like(labels)
     _launch(_abi.amb_mesh_component_sizes, 2, lp, n_faces, _ptr(sizes, torch.int32, "sizes", dev))
     return labels[:n_faces], sizes[:n_faces]
+
+
+# ---- multi-view normal rendering (csrc/render.cu) ----------------------------------------------------------------------------
+def _render_mesh(vertices: torch.Tensor, faces: torch.Tensor) -> tuple[int, int, int]:
+    """(current device, V, F) of a contiguous (V, 3) fp32 / (F, 3) int32 mesh."""
+    dev = _device(vertices, "vertices")
+    assert vertices.dim() == 2 and vertices.shape[1] == 3 and vertices.is_contiguous(), "vertices: expected a contiguous (V, 3) tensor"
+    return dev, vertices.shape[0], _mesh_faces(faces)
+
+
+def _cameras(cameras: torch.Tensor) -> int:
+    assert cameras.dim() == 2 and cameras.shape[1] == 12 and cameras.is_contiguous(), "cameras: expected a contiguous (C, 12) tensor"
+    return cameras.shape[0]
+
+
+def vertex_normals(vertices: torch.Tensor, faces: torch.Tensor) -> torch.Tensor:
+    """(V, 3) fp32 unit vertex normals: each vertex's sum of cross(v1 - v0, v2 - v0) over its faces in ascending face order,
+    over max(|n|, 1e-6).  Faces need three distinct corners (the vertex -> face lists come from amb_mesh_adjacency)."""
+    dev, V, F = _render_mesh(vertices, faces)
+    normals = torch.empty(V, 3, dtype=torch.float32, device=vertices.device)
+    if not F:
+        return normals.zero_()
+    work, scan = mesh_scan_scratch(V, F, vertices.device)
+    off = torch.empty(V + 1, dtype=torch.int32, device=vertices.device)
+    vf = torch.empty(3 * F, dtype=torch.int32, device=vertices.device)
+    nb = torch.empty(6 * F, dtype=torch.int32, device=vertices.device)
+    fp, adj = _ptr(faces, torch.int32, "faces", dev), _adjacency((off, vf, nb), dev)
+    _launch(_abi.amb_mesh_adjacency, 11, fp, F, V, _ptr(work, torch.int32, "work", dev), _ptr(scan, torch.int32, "scan", dev),
+            *adj)
+    _launch(_abi.amb_render_vertex_normals, 1, _ptr(vertices, torch.float32, "vertices", dev), V, fp, *adj[:2],
+            _ptr(normals, torch.float32, "normals", dev))
+    return normals
+
+
+def rasterize(vertices: torch.Tensor, faces: torch.Tensor, cameras: torch.Tensor, focal: float,
+              image_size: int) -> torch.Tensor:
+    """pix_to_face (C, 2S, 2S) int32 of the mesh seen by the (C, 12) cameras (R row-major, then T) at 2S x 2S samples: the
+    face with the smallest non-negative depth at each sample, ties to the lower index, -1 where none covers it."""
+    dev, V, F = _render_mesh(vertices, faces)
+    n_cams, n2 = _cameras(cameras), 2 * int(image_size)
+    d = vertices.device
+    keys = torch.empty(max(n_cams * n2 * n2, 1), dtype=torch.int64, device=d)
+    queue = torch.empty(n_cams * F + 1, dtype=torch.int32, device=d)
+    pix_to_face = torch.empty(n_cams, n2, n2, dtype=torch.int32, device=d)
+    _launch(_abi.amb_render_rasterize, 5 if F else 2, _ptr(vertices, torch.float32, "vertices", dev), V,
+            _ptr(faces, torch.int32, "faces", dev), F, _ptr(cameras, torch.float32, "cameras", dev), n_cams, float(focal),
+            int(image_size), _ptr(keys, torch.int64, "depth keys", dev), _ptr(queue, torch.int32, "queue", dev),
+            _ptr(pix_to_face, torch.int32, "pix_to_face", dev))
+    return pix_to_face
+
+
+def shade_normals(vertices: torch.Tensor, faces: torch.Tensor, normals: torch.Tensor, cameras: torch.Tensor, focal: float,
+                  pix_to_face: torch.Tensor, out: Optional[torch.Tensor] = None, column: int = 0) -> torch.Tensor:
+    """The composited normal images of `rasterize`'s views as uint8 RGB, view c written to the S x S cell at column
+    `column + c` of `out` (S, n_cols * S, 3) (allocated as (S, C * S, 3) when None) -> out."""
+    dev, V, F = _render_mesh(vertices, faces)
+    n_cams = _cameras(cameras)
+    assert pix_to_face.dim() == 3 and pix_to_face.shape[0] == n_cams and pix_to_face.shape[1] == pix_to_face.shape[2] \
+        and pix_to_face.shape[1] % 2 == 0 and pix_to_face.is_contiguous(), "pix_to_face: expected a contiguous (C, 2S, 2S) tensor"
+    assert normals.shape == vertices.shape and normals.is_contiguous(), "normals: expected a contiguous (V, 3) tensor"
+    S = pix_to_face.shape[1] // 2
+    if out is None:
+        out = torch.empty(S, n_cams * S, 3, dtype=torch.uint8, device=vertices.device)
+    assert out.dim() == 3 and out.shape[0] == S and out.shape[2] == 3 and out.stride(2) == 1 and out.stride(1) == 3 \
+        and 0 <= column and (column + n_cams) * S <= out.shape[1], "out: expected an (S, >= (column + C) * S, 3) row-major tensor"
+    cells = out[:, column * S:(column + n_cams) * S]
+    _launch(_abi.amb_render_shade_normals, 1, _ptr(vertices, torch.float32, "vertices", dev), V,
+            _ptr(faces, torch.int32, "faces", dev), F, _ptr(normals, torch.float32, "normals", dev),
+            _ptr(cameras, torch.float32, "cameras", dev), n_cams, float(focal), S,
+            _ptr(pix_to_face, torch.int32, "pix_to_face", dev), _ptr(cells, torch.uint8, "out", dev), out.stride(0), 3 * S)
+    return out

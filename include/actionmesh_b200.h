@@ -309,6 +309,37 @@ int amb_mesh_components(const int32_t* edges, int64_t n_edges, int64_t n_faces, 
                         amb_stream_t stream);
 int amb_mesh_component_sizes(const int32_t* labels, int64_t n_faces, int32_t* sizes, amb_stream_t stream);
 
+/* ---- multi-view normal rendering: vertex normals, rasterization, normal-image compositing (csrc/render.cu) ------------------
+ * Replaces ActionMeshVisualizer.render's per-view PyTorch3D calls (actionmesh/render/visualizer.py:109-141, renderer.py:87-185):
+ * Meshes.verts_normals_packed, MeshRasterizer (naive, bin_size=0, one face per pixel, blur 0, perspective-correct, clipped
+ * barycentrics, no culling, no z clip) at 2S x 2S samples, soft_normal_shading, the 2x2 average-pooled mask and
+ * make_normal_image's nearest reduction and white composite.  DESIGN.md §16 gives every formula; actionmesh_b200/render.py
+ * drives the calls.  All arithmetic is fp32 with each operation rounded on its own, in the order DESIGN.md states.
+ * vertices: (V, 3) fp32; faces: (F, 3) int32 in [0, V) (not checked on the device).  cameras: (C, 12) fp32 DEVICE array, R
+ * row-major then T, with X_view = X R + T (row vectors); focal is the focal length f, principal point 0.  V < 2^31 - 1 and
+ * 6F < 2^31.
+ *  render_vertex_normals: normals (V, 3) = each vertex's sum of cross(v1 - v0, v2 - v0) over its faces in ascending face order,
+ *    divided by max(|n|, 1e-6).  vf_offsets / vf_faces come from amb_mesh_adjacency on the same faces (which needs three
+ *    distinct corners per face).  Zero vertices launch nothing.
+ *  render_rasterize: pix_to_face (C, 2S, 2S) int32 = for each sample the face with the smallest non-negative depth, ties to the
+ *    lower index, -1 where none covers it.  depth_keys: C * 4 S^2 uint64 of scratch; queue: C * F + 1 int32 of scratch.
+ *    C * 4 S^2 and C * F must fit int32.  Zero faces give an all -1 pix_to_face (vertices and faces may then be NULL).  The
+ *    result does not depend on scheduling.
+ *  render_shade_normals: for each view c and output pixel (i, j) of S x S, the uint8 RGB of the composited normal image,
+ *    written at out + i * row_stride + c * view_stride + 3 j (+0, +1, +2) so the views land side by side in a grid row
+ *    (strides in bytes; view_stride >= 3 S when C > 1).  pix_to_face as written by render_rasterize with the same vertices,
+ *    faces, cameras, focal and S; normals as written by render_vertex_normals.  With zero faces every cell is white and
+ *    vertices, faces and normals may be NULL. */
+int amb_render_vertex_normals(const float* vertices, int64_t n_vertices, const int32_t* faces, const int32_t* vf_offsets,
+                              const int32_t* vf_faces, float* normals, amb_stream_t stream);
+int amb_render_rasterize(const float* vertices, int64_t n_vertices, const int32_t* faces, int64_t n_faces,
+                         const float* cameras, int n_cameras, float focal, int image_size, uint64_t* depth_keys,
+                         int32_t* queue, int32_t* pix_to_face, amb_stream_t stream);
+int amb_render_shade_normals(const float* vertices, int64_t n_vertices, const int32_t* faces, int64_t n_faces,
+                             const float* normals, const float* cameras, int n_cameras, float focal, int image_size,
+                             const int32_t* pix_to_face, uint8_t* out, int64_t row_stride, int64_t view_stride,
+                             amb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
