@@ -742,3 +742,89 @@ def shade_normals(vertices: torch.Tensor, faces: torch.Tensor, normals: torch.Te
             _ptr(cameras, torch.float32, "cameras", dev), n_cams, float(focal), S,
             _ptr(pix_to_face, torch.int32, "pix_to_face", dev), _ptr(cells, torch.uint8, "out", dev), out.stride(0), 3 * S)
     return out
+
+
+def _icp_tensor(t: torch.Tensor, shape: tuple, name: str) -> None:
+    if tuple(t.shape) != shape or not t.is_contiguous():
+        raise _lib.AmbError(f"{name}: expected a contiguous {shape} tensor, got {tuple(t.shape)}")
+
+
+def icp_scratch_doubles(frames: int, candidates: int, n_pred: int, n_gt: int) -> int:
+    """Size in fp64 elements of the scratch `icp_chamfer_grad` needs for these sizes."""
+    n = C.c_int64()
+    _lib.check(_abi.amb_icp_scratch_doubles(int(frames), int(candidates), int(n_pred), int(n_gt), C.byref(n)),
+               "amb_icp_scratch_doubles")
+    return n.value
+
+
+def icp_chamfer_grad(pred: torch.Tensor, gt: torch.Tensor, rot: torch.Tensor, params: torch.Tensor,
+                     out: Optional[torch.Tensor] = None, scratch: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Chamfer loss and gradient sums of every (frame, candidate) transform -> (F, C, 13) fp64 = loss, t (3), A (3x3).
+
+    pred (F, P, 3), gt (F, Q, 3) fp32; rot (F, C, 3, 3) and params (F, C, 12) = T, d6, s fp32.  The prediction under a
+    candidate is (s * x) @ R + T; see include/actionmesh_b200.h for t and A."""
+    dev = _device(pred, "pred")
+    if pred.dim() != 3 or gt.dim() != 3 or pred.shape[2] != 3 or gt.shape[2] != 3 or gt.shape[0] != pred.shape[0]:
+        raise _lib.AmbError(f"icp_chamfer_grad: expected (F, P, 3) and (F, Q, 3) points, got {tuple(pred.shape)} and "
+                            f"{tuple(gt.shape)}")
+    F, P, Q, nc = pred.shape[0], pred.shape[1], gt.shape[1], params.shape[1] if params.dim() == 3 else 0
+    _icp_tensor(pred, (F, P, 3), "pred")
+    _icp_tensor(gt, (F, Q, 3), "gt")
+    _icp_tensor(rot, (F, nc, 3, 3), "rot")
+    _icp_tensor(params, (F, nc, 12), "params")
+    need = icp_scratch_doubles(F, nc, P, Q)
+    if scratch is None:
+        scratch = torch.empty(need, dtype=torch.float64, device=pred.device)
+    elif scratch.numel() < need:
+        raise _lib.AmbError(f"icp_chamfer_grad: scratch holds {scratch.numel()} doubles, {need} needed")
+    if out is None:
+        out = torch.empty(F, nc, 13, dtype=torch.float64, device=pred.device)
+    _icp_tensor(out, (F, nc, 13), "out")
+    _launch(_abi.amb_icp_chamfer_grad, 2, _ptr(pred, torch.float32, "pred", dev), _ptr(gt, torch.float32, "gt", dev), F, nc,
+            P, Q, _ptr(rot, torch.float32, "rot", dev), _ptr(params, torch.float32, "params", dev),
+            _ptr(scratch, torch.float64, "scratch", dev), _ptr(out, torch.float64, "out", dev),
+            tag="icp_chamfer_grad", meta=(F, nc, P, Q))
+    return out
+
+
+def icp_adam_step(sums: torch.Tensor, rot_init: torch.Tensor, step: int, lr: float, params: torch.Tensor,
+                  adam_m: torch.Tensor, adam_v: torch.Tensor, rot: torch.Tensor, best: torch.Tensor) -> None:
+    """Adam step `step` (1-based) of every (frame, candidate) from `icp_chamfer_grad`'s sums, in place on params, adam_m,
+    adam_v (F, C, 12) and rot (F, C, 3, 3), with the best candidate so far tracked in best (F, 16) = loss, R, T, s."""
+    dev = _device(sums, "sums")
+    if sums.dim() != 3:
+        raise _lib.AmbError(f"icp_adam_step: expected (F, C, 13) sums, got {tuple(sums.shape)}")
+    F, nc = sums.shape[0], sums.shape[1]
+    _icp_tensor(sums, (F, nc, 13), "sums")
+    _icp_tensor(rot_init, (nc, 3, 3), "rot_init")
+    for t, name in ((params, "params"), (adam_m, "adam_m"), (adam_v, "adam_v")):
+        _icp_tensor(t, (F, nc, 12), name)
+    _icp_tensor(rot, (F, nc, 3, 3), "rot")
+    _icp_tensor(best, (F, 16), "best")
+    if step < 1:
+        raise _lib.AmbError(f"icp_adam_step: step {step} < 1")
+    if rot.data_ptr() == rot_init.data_ptr():
+        raise _lib.AmbError("icp_adam_step: rot must not alias rot_init (the step overwrites rot)")
+    # torch.optim.Adam computes these scalars in double on the host and applies them to the fp32 state
+    step_size = -(float(lr) / (1 - 0.9 ** step))
+    bias2_sqrt = (1 - 0.999 ** step) ** 0.5
+    _launch(_abi.amb_icp_adam_step, 1, _ptr(sums, torch.float64, "sums", dev), _ptr(rot_init, torch.float32, "rot_init", dev),
+            F, nc, step_size, bias2_sqrt, _ptr(params, torch.float32, "params", dev),
+            _ptr(adam_m, torch.float32, "adam_m", dev), _ptr(adam_v, torch.float32, "adam_v", dev),
+            _ptr(rot, torch.float32, "rot", dev), _ptr(best, torch.float32, "best", dev), tag="icp_adam_step", meta=(F, nc))
+
+
+def icp_transform_points(points: torch.Tensor, transform: torch.Tensor) -> torch.Tensor:
+    """(F, N, 3) fp32 points -> (s * p) @ R + T as pytorch3d's composed Scale / Rotate / Translate applies it, with
+    transform (F, 15) or (1, 15) = R (9), T (3), s (3) per frame ((1, 15): the same transform for every frame)."""
+    dev = _device(points, "points")
+    if points.dim() != 3 or points.shape[2] != 3 or transform.dim() != 2 or transform.shape[1] != 15 \
+            or transform.shape[0] not in (1, points.shape[0]) or transform.stride(1) != 1:
+        raise _lib.AmbError(f"icp_transform_points: expected (F, N, 3) points and an (F | 1, 15) transform, got "
+                            f"{tuple(points.shape)} and {tuple(transform.shape)}")
+    p = points.contiguous()
+    out = torch.empty_like(p)
+    stride = transform.stride(0) if transform.shape[0] > 1 else 0
+    _launch(_abi.amb_icp_transform_points, 1 if p.numel() else 0, _ptr(p, torch.float32, "points", dev), p.shape[0],
+            p.shape[1], _ptr(transform, torch.float32, "transform", dev), stride, _ptr(out, torch.float32, "out", dev))
+    return out

@@ -106,6 +106,35 @@ int amb_composite_crop_pad(const uint8_t* rgba, int n_images, int height, int wi
 int amb_nearest_neighbors(const float* query, int n_query, const float* reference, int n_reference, void* scratch_u64,
                           float* out_dist, int32_t* out_index, amb_stream_t stream);
 
+/* ---- ActionBench gradient ICP (csrc/icp.cu; SURVEY 8(f) rank 4) --------------------------------------------------------
+ * Replaces the optimisation loop of gradient_icp (actionbench/icp.py:53-112) for F frames x C candidates at once (the
+ * reference: one frame, C = 24).  pred: (F, P, 3) fp32, gt: (F, Q, 3) fp32.  Per (frame f, candidate n): rot (F, C, 9) = R
+ * row-major; params (F, C, 12) fp32 = T (3), the 6D rotation d6 (6), s (3), in torch.optim.Adam's parameter order; the
+ * prediction is y_i = (s * x_i) @ R + T (row vectors).  1 <= C <= 1024; F, P, Q >= 1.
+ *  icp_scratch_doubles: the fp64 scratch icp_chamfer_grad needs for these sizes.
+ *  icp_chamfer_grad: sums (F, C, 13) fp64 = the loss L = (1/P) sum_i min_j |y_i - g_j|^2 + (1/Q) sum_j min_i |y_i - g_j|^2
+ *    (pytorch3d chamfer_distance, batch_reduction=None), then t = sum G (3) and A = sum x ⊗ G (3x3 row-major, over the
+ *    untransformed x), where G = (2/P)(y_i - g_a(i)) for every pred point (a(i): nearest gt point) and (2/Q)(y_b(j) - g_j),
+ *    paired with x_b(j), for every gt point (b(j): nearest prediction).  Ties go to the lowest index.  The result does not
+ *    depend on scheduling (no float atomics).
+ *  icp_adam_step: with those sums, dL/dT = t, dL/dR[k,l] = s_k A[k,l], dL/ds_k = sum_l R[k,l] A[k,l], all scaled by 1/C
+ *    (the reference back-propagates the mean over candidates), back-propagated through R = rot_init (C, 9) @
+ *    rotation_6d_to_matrix(d6); one torch.optim.Adam step (defaults) on params with moments adam_m, adam_v (F, C, 12) fp32,
+ *    where step_size = -lr / (1 - 0.9^t) and bias2_sqrt = sqrt(1 - 0.999^t) for step t >= 1; best (F, 16) fp32 = loss, R (9),
+ *    T (3), s (3) of the best candidate so far, updated as icp.py:99-106 does (init loss = +inf); rot is overwritten with R of
+ *    the updated params.
+ *  icp_transform_points: points (F, n_points, 3) fp32 -> out = p @ M + T with M[k,l] = s_k R[k,l] (fp32, the matrix product
+ *    pytorch3d's Scale(s).compose(Rotate(R), Translate(T)).transform_points applies); transform holds R (9), T (3), s (3) of
+ *    frame f at transform + f * transform_stride (stride 0: one transform for every frame).  frames <= 65535. */
+int amb_icp_scratch_doubles(int frames, int candidates, int n_pred, int n_gt, int64_t* out_doubles);
+int amb_icp_chamfer_grad(const float* pred, const float* gt, int frames, int candidates, int n_pred, int n_gt,
+                         const float* rot, const float* params, double* scratch, double* sums, amb_stream_t stream);
+int amb_icp_adam_step(const double* sums, const float* rot_init, int frames, int candidates, float step_size,
+                      float bias2_sqrt, float* params, float* adam_m, float* adam_v, float* rot, float* best,
+                      amb_stream_t stream);
+int amb_icp_transform_points(const float* points, int frames, int64_t n_points, const float* transform,
+                             int64_t transform_stride, float* out, amb_stream_t stream);
+
 /* ---- Stage II (temporal autoencoder) helpers — first "next" row of SURVEY 8(f) -----------------------------------------
  * alpha_rows: the (source_alpha, target_alpha) token of actionmesh/model/temporal_autoencoder.py:233-237 (TimestepEmbedder,
  *   model/utils/embeddings.py:56-132), fp32, written to n_rows rows `row_stride` elements apart.
