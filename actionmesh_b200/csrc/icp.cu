@@ -312,8 +312,12 @@ __global__ void icp_adam_kernel(const double* __restrict__ sums, const float* __
     for (int k = 0; k < 3; ++k)
       grad[9 + k] = (double)r_old[3 * k] * A[3 * k] + (double)r_old[3 * k + 1] * A[3 * k + 1] + (double)r_old[3 * k + 2] * A[3 * k + 2];
     rot6d_backward(par + 3, gm, grad + 3);
-    // 3. torch.optim.Adam (defaults: betas 0.9 / 0.999, eps 1e-8), the fp32 operations of its foreach path:
-    //    m = lerp(m, g, 0.1); v = v * 0.999 + 0.001 g g; p += step_size * m / (sqrt(v) / bias2_sqrt + eps),
+    // 3. torch.optim.Adam (defaults: betas 0.9 / 0.999, eps 1e-8) in fp32:
+    //    m = lerp(m, g, 0.1) = fma(0.1, g - m, m), as both of torch's paths compute it;
+    //    v = fma(fl(0.001 g), g, fl(0.999 v)), the order of torch's CPU path (fl(fl(0.001 g) g) + fl(0.999 v)), whose
+    //      results it gives on the tested inputs; torch's CUDA path computes fma(0.001, fl(g g), fl(0.999 v)) instead
+    //      (DESIGN §12 says why the CPU order is kept);
+    //    p = fma(step_size, m / denom, p) with denom = sqrt(v) / bias2_sqrt + eps, as torch's CUDA path computes it,
     //    step_size = -lr / (1 - 0.9^t) and bias2_sqrt = sqrt(1 - 0.999^t) computed in double by the caller.
     for (int e = 0; e < 12; ++e) {
       const float g = (float)grad[e];

@@ -3,8 +3,9 @@ sample_point_cloud}.py).
 
 Same functions, arguments, subsampling (numpy RandomState(seed) / (seed + 1) permutations) and return values as
 `compute_chamfer_score` (chamfer.py:12-53) and `compute_motion_chamfer_score` (:56-89); the KD-tree nearest-neighbour queries
-run as a brute-force CUDA search (amb_nearest_neighbors).  Distances are fp32 (the KD-tree works in fp64): the scores agree to
-~1e-6 relative, see tests/test_evaluation_gpu.py.
+run as a brute-force CUDA search (amb_nearest_neighbors).  Distances are fp32 and equal an exact fp32 restatement bit for
+bit, ties to the lowest index (tests/test_icp_exact_gpu.py); against the KD-tree's fp64 the scores agree to <= 1e-5
+relative (tests/test_evaluation_gpu.py).
 
 `gradient_icp` / `gradient_icp_frames` restate icp.py:53-112 on two kernels per Adam step (csrc/icp.cu, DESIGN §12): the
 Chamfer loss and its gradient sums, then the closed-form backward, Adam and best-candidate tracking.  The host enqueues the

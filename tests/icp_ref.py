@@ -5,7 +5,7 @@ Not collected by pytest.  Everything takes and returns CPU tensors:
   * `chamfer_sums` — the loss and the 12 gradient sums t, A of every candidate, from explicit nearest-neighbour choices;
   * `rot6d_to_matrix` / `rot6d_backward` — pytorch3d's 6D rotation and the closed-form backward the kernel uses;
   * `param_grads` — dL/d(T, d6, s) of loss.mean() over the candidates from the sums;
-  * `adam_step` — torch.optim.Adam's update at its defaults, fp32;
+  * `adam_step` — torch.optim.Adam's update at its defaults, fp32, to a few ulps;
   * `best_update` — icp.py:99-106's bookkeeping (pre-step R, post-step T and s; NaN anywhere records nothing).
 """
 from __future__ import annotations
@@ -99,7 +99,9 @@ def param_grads(sums: torch.Tensor, rot_init: torch.Tensor, R: torch.Tensor, par
 
 
 def adam_step(params, m, v, grad, step: int, lr: float):
-    """torch.optim.Adam (betas 0.9 / 0.999, eps 1e-8) on fp32 tensors -> new (params, m, v)."""
+    """torch.optim.Adam (betas 0.9 / 0.999, eps 1e-8) on fp32 tensors -> new (params, m, v).  m and v in the order of
+    torch's CPU path (v = fl(0.999 v) + fl(fl(0.001 g) g)); torch's CUDA path computes v = fma(0.001, fl(g g), fl(0.999 v)),
+    and the params update rounds differently on both, so this is an approximation to a few ulps (DESIGN §12)."""
     grad = grad.float()
     m = torch.lerp(m, grad, 1 - 0.9)
     v = v * 0.999 + (1 - 0.999) * grad * grad
