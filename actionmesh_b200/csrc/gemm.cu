@@ -148,6 +148,9 @@ __device__ __forceinline__ float2 finish_pair(const GemmParams& p, float v0, flo
   if (p.act == 1) {
     v0 = gelu_erf(v0);
     v1 = gelu_erf(v1);
+  } else if (p.act == 2) {  // ReLU (RMBG's REBNCONV, csrc/rmbg.cu)
+    v0 = fmaxf(v0, 0.f);
+    v1 = fmaxf(v1, 0.f);
   }
   if (p.col_scale) {
     const float2 s = __ldg(reinterpret_cast<const float2*>(p.col_scale + col));
@@ -563,7 +566,7 @@ extern "C" int amb_gemm_bf16(const amb_gemm_args* a, amb_stream_t stream) {
   AMB_CHECK_ARG(!a->a2 || (a->k_split > 0 && a->k_split < a->k && a->k_split % BK == 0 && a->lda2 % 8 == 0),
                 "gemm: bad k_split %d", a->k_split);
   AMB_CHECK_ARG(!a->residual || a->ldr % 8 == 0, "gemm: ldr must be a multiple of 8");
-  AMB_CHECK_ARG(a->act == 0 || a->act == 1, "gemm: unknown activation %d", a->act);
+  AMB_CHECK_ARG(a->act >= 0 && a->act <= 2, "gemm: unknown activation %d", a->act);
   AMB_CHECK_ARG(!a->c2 || a->ldc2 % 8 == 0, "gemm: ldc2 must be a multiple of 8");
   // the epilogue writes (and reads the residual in) 8-column, 16-byte vectors
   AMB_CHECK_ARG((uintptr_t)a->c % 16 == 0 && (uintptr_t)a->c2 % 16 == 0 && (uintptr_t)a->residual % 16 == 0,

@@ -828,3 +828,125 @@ def icp_transform_points(points: torch.Tensor, transform: torch.Tensor) -> torch
     _launch(_abi.amb_icp_transform_points, 1 if p.numel() else 0, _ptr(p, torch.float32, "points", dev), p.shape[0],
             p.shape[1], _ptr(transform, torch.float32, "transform", dev), stride, _ptr(out, torch.float32, "out", dev))
     return out
+
+
+# ---- background removal: RMBG-1.4's resampling, im2col, mask head and refinement (csrc/rmbg.cu) ------------------------------
+# Activations are fp32 NHWC feature maps held as 2-D (H * W, pixel stride) tensors with unit channel stride: a GEMM output
+# padded to 64 columns is read in place, its first C columns being the channels.
+def _feature_map(t: torch.Tensor, h: int, w: int, c: int, name: str) -> None:
+    if t.dim() != 2 or t.shape[0] != h * w or t.stride(1) != 1 or t.shape[1] < c or (h * w > 1 and t.stride(0) < c):
+        raise _lib.AmbError(f"{name}: expected a ({h * w}, >= {c}) feature map with unit channel stride, got "
+                            f"{tuple(t.shape)} strides {t.stride()}")
+
+
+def _contiguous(t: torch.Tensor, shape: tuple, name: str) -> None:
+    if tuple(t.shape) != tuple(shape) or not t.is_contiguous():
+        raise _lib.AmbError(f"{name}: expected a contiguous {tuple(shape)} tensor, got {tuple(t.shape)}")
+
+
+def conv3x3_out(size: int, stride: int, pad: int, dilation: int) -> int:
+    return (size + 2 * pad - 2 * dilation - 1) // stride + 1
+
+
+def rmbg_resize_input(rgb: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """(H, W, 3) uint8 frame -> out (S_h, S_w, 3) fp32 = bilinear(frame) / 255 - 0.5 (background_removal.py:57-69)."""
+    dev = _device(rgb, "rgb")
+    if rgb.dim() != 3 or rgb.shape[2] != 3:
+        raise _lib.AmbError(f"rmbg_resize_input: expected an (H, W, 3) frame, got {tuple(rgb.shape)}")
+    _contiguous(rgb, rgb.shape, "rgb")
+    if out.dim() != 3:
+        raise _lib.AmbError(f"rmbg_resize_input: expected an (S_h, S_w, 3) output, got {tuple(out.shape)}")
+    _contiguous(out, (out.shape[0], out.shape[1], 3), "out")
+    _launch(_abi.amb_rmbg_resize_input, 1, _ptr(rgb, torch.uint8, "rgb", dev), rgb.shape[0], rgb.shape[1],
+            _ptr(out, torch.float32, "out", dev), out.shape[0], out.shape[1], tag="rmbg_resize")
+    return out
+
+
+def rmbg_im2col_split(sources: list, h: int, w: int, out: torch.Tensor, *, stride: int = 1, pad: int = 1,
+                      dilation: int = 1) -> torch.Tensor:
+    """3x3 patches of the channel concatenation of `sources` = [(feature map, channels)] (one or two) -> out
+    (H_o * W_o, 3 k_pad) bf16 in split3's activation layout [hi | lo | hi], k_pad = out.shape[1] / 3."""
+    dev = _device(out, "out")
+    if not 1 <= len(sources) <= 2:
+        raise _lib.AmbError(f"rmbg_im2col_split: one or two sources, got {len(sources)}")
+    for i, (t, c) in enumerate(sources):
+        _feature_map(t, h, w, c, f"source {i}")
+    rows = conv3x3_out(h, stride, pad, dilation) * conv3x3_out(w, stride, pad, dilation)
+    if out.dim() != 2 or out.stride(1) != 1 or out.shape[0] != rows or out.shape[1] % 3:
+        raise _lib.AmbError(f"rmbg_im2col_split: expected a ({rows}, 3 k_pad) output, got {tuple(out.shape)}")
+    (s0, c0), (s1, c1) = sources[0], (sources[1] if len(sources) == 2 else (None, 0))
+    _launch(_abi.amb_rmbg_im2col_split, 1, _ptr(s0, torch.float32, "source 0", dev), int(c0), s0.stride(0),
+            _ptr(s1, torch.float32, "source 1", dev), int(c1), s1.stride(0) if s1 is not None else 0, h, w, stride, pad,
+            dilation, out.shape[1] // 3, _ptr(out, torch.bfloat16, "out", dev), out.stride(0), tag="rmbg_im2col",
+            meta=(rows, out.shape[1] // 3))
+    return out
+
+
+def rmbg_maxpool2(src: torch.Tensor, h: int, w: int, c: int, out: torch.Tensor) -> torch.Tensor:
+    """MaxPool2d(2, 2, ceil_mode=True) of an (h, w, c) feature map -> out (ceil(h/2) * ceil(w/2), >= c)."""
+    dev = _device(src, "src")
+    _feature_map(src, h, w, c, "src")
+    _feature_map(out, (h + 1) // 2, (w + 1) // 2, c, "out")
+    _launch(_abi.amb_rmbg_maxpool2, 1, _ptr(src, torch.float32, "src", dev), src.stride(0), h, w, c,
+            _ptr(out, torch.float32, "out", dev), out.stride(0), tag="rmbg_pool")
+    return out
+
+
+def rmbg_upsample(src: torch.Tensor, h: int, w: int, c: int, out: torch.Tensor, out_h: int, out_w: int) -> torch.Tensor:
+    """Bilinear (align_corners=False) resize of an (h, w, c) feature map to out (out_h * out_w, >= c)."""
+    dev = _device(src, "src")
+    _feature_map(src, h, w, c, "src")
+    _feature_map(out, out_h, out_w, c, "out")
+    _launch(_abi.amb_rmbg_upsample, 1, _ptr(src, torch.float32, "src", dev), src.stride(0), h, w, c,
+            _ptr(out, torch.float32, "out", dev), out.stride(0), out_h, out_w, tag="rmbg_upsample")
+    return out
+
+
+def rmbg_mask_head(feat: torch.Tensor, h: int, w: int, weight: torch.Tensor, model_size: tuple, out_size: tuple,
+                   work: Optional[dict] = None) -> dict:
+    """side1 on the (h, w, 64) stage1d features -> dict(logits (h, w), soft (S_h, S_w) = sigmoid(d1), resized (H, W),
+    mask (H, W) uint8) as _postprocess_mask computes it; `work` may hold those tensors (and minmax) to reuse."""
+    dev = _device(feat, "feat")
+    _feature_map(feat, h, w, 64, "feat")
+    _contiguous(weight, (577,), "weight")
+    (sh, sw), (oh, ow) = (int(v) for v in model_size), (int(v) for v in out_size)
+    work = {} if work is None else work
+    for name, shape, dt in (("logits", (h, w), torch.float32), ("soft", (sh, sw), torch.float32),
+                            ("resized", (oh, ow), torch.float32), ("mask", (oh, ow), torch.uint8),
+                            ("minmax", (2,), torch.int32)):
+        if name not in work:
+            work[name] = torch.empty(shape, dtype=dt, device=feat.device)
+        _contiguous(work[name], shape, name)
+    _launch(_abi.amb_rmbg_mask_head, 4, _ptr(feat, torch.float32, "feat", dev), feat.stride(0), h, w,
+            _ptr(weight, torch.float32, "weight", dev), _ptr(work["logits"], torch.float32, "logits", dev), sh, sw,
+            _ptr(work["soft"], torch.float32, "soft", dev), oh, ow, _ptr(work["resized"], torch.float32, "resized", dev),
+            _ptr(work["minmax"], torch.int32, "minmax", dev), _ptr(work["mask"], torch.uint8, "mask", dev),
+            tag="rmbg_mask_head")
+    return work
+
+
+def rmbg_refine_rgba(rgb: torch.Tensor, mask: torch.Tensor, refine: bool = True, min_size: int = 200,
+                     out: Optional[torch.Tensor] = None, work: Optional[dict] = None) -> torch.Tensor:
+    """(H, W, 3) uint8 frame + (H, W) uint8 mask -> (H, W, 4) RGBA with alpha = refine_mask(mask, min_size) (Otsu, 8-connected
+    components of >= min_size pixels, 0 / 255) or the mask itself.  `work` receives hist (257: histogram, Otsu threshold),
+    labels and sizes (H * W int32 each: component root per foreground pixel, -1 elsewhere; pixels per root)."""
+    dev = _device(rgb, "rgb")
+    if rgb.dim() != 3 or rgb.shape[2] != 3:
+        raise _lib.AmbError(f"rmbg_refine_rgba: expected an (H, W, 3) frame, got {tuple(rgb.shape)}")
+    H, W = rgb.shape[0], rgb.shape[1]
+    _contiguous(rgb, (H, W, 3), "rgb")
+    _contiguous(mask, (H, W), "mask")
+    if out is None:
+        out = torch.empty(H, W, 4, dtype=torch.uint8, device=rgb.device)
+    _contiguous(out, (H, W, 4), "out")
+    work = {} if work is None else work
+    if refine:
+        for name, n in (("hist", 257), ("labels", H * W), ("sizes", H * W)):
+            if name not in work:
+                work[name] = torch.empty(n, dtype=torch.int32, device=rgb.device)
+            _contiguous(work[name], (n,), name)
+    get = lambda name: _ptr(work[name], torch.int32, name, dev) if refine else None
+    _launch(_abi.amb_rmbg_refine_rgba, 6 if refine else 1, _ptr(rgb, torch.uint8, "rgb", dev),
+            _ptr(mask, torch.uint8, "mask", dev), H, W, int(bool(refine)), int(min_size), get("hist"), get("labels"),
+            get("sizes"), _ptr(out, torch.uint8, "out", dev), tag="rmbg_refine")
+    return out

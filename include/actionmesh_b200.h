@@ -182,7 +182,7 @@ typedef struct amb_gemm_args {
   const void* residual; /* (m', n) bf16/fp32 or NULL; added after the activation; may alias c */
   int64_t ldr;
   int32_t res_fp32;
-  int32_t act;          /* 0 none, 1 GELU(erf) */
+  int32_t act;          /* 0 none, 1 GELU(erf), 2 ReLU (RMBG's REBNCONV, briarmbg.py:24) */
   const float* col_scale; /* (n) or NULL: per-column scale applied after bias/act, before residual (DinoV2 LayerScale) */
   /* output row remap: dst_row = (row / grp_rows) * grp_stride + row % grp_rows + row_off  (grp_rows == 0: identity) */
   int32_t grp_rows, grp_stride, row_off;
@@ -368,6 +368,47 @@ int amb_render_shade_normals(const float* vertices, int64_t n_vertices, const in
                              const float* normals, const float* cameras, int n_cameras, float focal, int image_size,
                              const int32_t* pix_to_face, uint8_t* out, int64_t row_stride, int64_t view_stride,
                              amb_stream_t stream);
+
+/* ---- background removal: RMBG-1.4 around split-bf16 GEMM convolutions, mask head and refinement (csrc/rmbg.cu) -------------
+ * Replaces BackgroundRemover.forward (actionmesh/preprocessing/background_removal.py:84-112) with BriaRMBG
+ * (third_party/TripoSG/scripts/briarmbg.py:355-463).  Every 3x3 convolution is rmbg_im2col_split followed by amb_gemm_bf16 on
+ * the split operand (BN folded into the weights, act 2, the RSU residual as the GEMM residual); DESIGN.md §17 and
+ * actionmesh_b200/background_removal.py drive the calls.  Activations are fp32 NHWC: pixel p, channel c at p * ps + c, with a
+ * pixel stride ps >= the channel count.  Bilinear resampling is align_corners=False with scale = in / out in fp32, src =
+ * max(scale (dst + 0.5) - 0.5, 0) and h0 (w0 x00 + w1 x01) + h1 (w0 x10 + w1 x11), every operation rounded on its own.
+ * Images are at most 2^30 pixels.
+ *  rmbg_resize_input: uint8 RGB (height, width, 3) -> fp32 (out_height, out_width, 3) = bilinear / 255 - 0.5 (_preprocess_image,
+ *    background_removal.py:57-69).
+ *  rmbg_im2col_split: the 3x3 patches (stride 1 or 2, dilation d, padding <= d) of the channel concatenation [src0 | src1]
+ *    (src1 NULL when c1 = 0; replaces the RSU decoders' torch.cat, briarmbg.py:99-114) -> bf16 rows (out_h * out_w, ld_dst)
+ *    with columns (ky, kx, c) zero-padded to k_pad (a multiple of 64), written as amb_split3_bf16's activation layout
+ *    [hi | lo | hi] with seg = k_pad.  out_h = (height + 2 pad - 2 d - 1) / stride + 1.
+ *  rmbg_maxpool2: MaxPool2d(2, stride=2, ceil_mode=True) (briarmbg.py:49) -> (ceil(h / 2), ceil(w / 2), channels).
+ *  rmbg_upsample: _upsample_like (briarmbg.py:29-33) to (out_height, out_width).
+ *  rmbg_mask_head: side1 (3x3, 64 -> 1, bias; weight = 576 fp32 in (ky, kx, c) order, then the bias) on the stage1d features
+ *    -> logits (height, width); soft = sigmoid(upsample(logits)) at the model size (result[0][0], briarmbg.py:445-446,463);
+ *    resized = upsample(soft) at the frame size, and mask = uint8((resized - min) / (max - min) * 255), truncated
+ *    (_postprocess_mask, background_removal.py:71-82).  When max == min the reference divides by zero; mask is then all 0.
+ *    minmax: 2 int32 of scratch.  feat 16-byte aligned with ps >= 64, a multiple of 4.
+ *  rmbg_refine_rgba: rgba (height, width, 4) = the RGB frame with alpha = mask (refine 0) or refine_mask(mask, min_size)
+ *    (refine 1, background_removal.py:20-38): cv2's Otsu threshold t (in double, as OpenCV computes it), foreground mask > t,
+ *    8-connected components, components of fewer than min_size pixels dropped, 0 / 255.  hist: 257 int32 (the histogram, then
+ *    t); labels, sizes: height * width int32 (each foreground pixel's component root = its smallest pixel index, and each
+ *    root's pixel count).  The result does not depend on scheduling.
+ */
+int amb_rmbg_resize_input(const uint8_t* rgb, int height, int width, float* out, int out_height, int out_width,
+                          amb_stream_t stream);
+int amb_rmbg_im2col_split(const float* src0, int c0, int64_t ps0, const float* src1, int c1, int64_t ps1, int height, int width,
+                          int stride, int pad, int dilation, int k_pad, void* dst_bf16, int64_t ld_dst, amb_stream_t stream);
+int amb_rmbg_maxpool2(const float* src, int64_t ps_src, int height, int width, int channels, float* dst, int64_t ps_dst,
+                      amb_stream_t stream);
+int amb_rmbg_upsample(const float* src, int64_t ps_src, int height, int width, int channels, float* dst, int64_t ps_dst,
+                      int out_height, int out_width, amb_stream_t stream);
+int amb_rmbg_mask_head(const float* feat, int64_t ps, int height, int width, const float* weight, float* logits, int model_height,
+                       int model_width, float* soft, int out_height, int out_width, float* resized, int32_t* minmax,
+                       uint8_t* mask, amb_stream_t stream);
+int amb_rmbg_refine_rgba(const uint8_t* rgb, const uint8_t* mask, int height, int width, int refine, int min_size,
+                         int32_t* hist, int32_t* labels, int32_t* sizes, uint8_t* rgba, amb_stream_t stream);
 
 #ifdef __cplusplus
 }
