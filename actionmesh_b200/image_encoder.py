@@ -21,6 +21,7 @@ image (actionmesh_b200/preprocess.py); `image_preprocess_dino` keeps the HF obje
 """
 from __future__ import annotations
 
+import json
 import math
 import os
 from typing import List, Optional
@@ -44,6 +45,34 @@ def default_preprocessor():
                              crop_size={"height": 224, "width": 224}, do_rescale=True, rescale_factor=1 / 255.0,
                              do_normalize=True, image_mean=list(IMAGENET_MEAN), image_std=list(IMAGENET_STD),
                              do_convert_rgb=True)
+
+
+def hf_dinov2_arguments(model_dir: str, feature_extractor_dir: str) -> dict:
+    """B200ImageEncoder's shape arguments for an HF `Dinov2Model` directory and its `BitImageProcessor` directory.
+
+    `Dinov2Config` does not name things the way the constructor does, so `B200Module.from_pretrained`'s match by name would
+    go wrong: `num_hidden_layers` / `num_attention_heads` are `num_layers` / `num_heads`, and its `image_size` is the grid
+    the position embeddings were trained at (518 for dinov2-large), not the input size.  The input size is the feature
+    extractor's crop, the size `B200ImagePreprocessor.from_hf` produces; it must be square and a multiple of the patch."""
+    from transformers import BitImageProcessor
+
+    from .preprocess import B200ImagePreprocessor
+
+    for d, name in ((model_dir, "config.json"), (feature_extractor_dir, "preprocessor_config.json")):
+        if not os.path.isfile(os.path.join(d, name)):
+            raise AmbError(f"B200ImageEncoder: {os.path.join(d, name)} not found")
+    with open(os.path.join(model_dir, "config.json")) as f:
+        cfg = json.load(f)
+    if cfg.get("use_swiglu_ffn", False) or cfg.get("hidden_act", "gelu") != "gelu":
+        raise AmbError("B200ImageEncoder: only DinoV2's GELU MLP is supported")
+    patch = int(cfg.get("patch_size", 14))
+    ch, cw = B200ImagePreprocessor.from_hf(BitImageProcessor.from_pretrained(feature_extractor_dir)).crop_size
+    if ch != cw or ch % patch:
+        raise AmbError(f"B200ImageEncoder: the crop {ch}x{cw} of {feature_extractor_dir} must be square and a multiple of "
+                       f"patch_size {patch}")
+    return dict(hidden_size=int(cfg.get("hidden_size", 1024)), num_layers=int(cfg["num_hidden_layers"]),
+                num_heads=int(cfg["num_attention_heads"]), patch_size=patch, image_size=ch,
+                mlp_ratio=int(cfg.get("mlp_ratio", 4)), layer_norm_eps=float(cfg.get("layer_norm_eps", 1e-6)))
 
 
 class B200ImageEncoder(B200Module):
@@ -77,6 +106,13 @@ class B200ImageEncoder(B200Module):
             self.image_preprocess_dino = default_preprocessor()
         if pretrained_dino_model is not None:
             self._pending_sd = read_weights(pretrained_dino_model, self.weight_files)
+
+    @classmethod
+    def from_hf_dirs(cls, model_dir: str, feature_extractor_dir: str, precision: str = "fp32", device="cuda"):
+        """An HF `Dinov2Model` directory (config.json + weights) and its `BitImageProcessor` directory
+        (preprocessor_config.json), loaded onto `device`; the constructor arguments are `hf_dinov2_arguments`'."""
+        return cls(feature_extractor_dir, model_dir, precision=precision,
+                   **hf_dinov2_arguments(model_dir, feature_extractor_dir)).to(device)
 
     def _after_to(self, moved: bool) -> None:
         """The weights of `pretrained_dino_model` are packed on the first `to()`."""

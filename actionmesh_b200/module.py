@@ -25,6 +25,17 @@ def read_weights(path: str, names) -> dict:
     return torch.load(file, map_location="cpu")
 
 
+def check_files(root: str, required, what: str) -> None:
+    """`required`: (subdirectory, file names) pairs; each subdirectory of `root` must hold one of its names.  Raises one
+    AmbError naming the first path that is missing (a subdirectory, or its preferred file name)."""
+    for sub, names in required:
+        d = os.path.join(root, sub)
+        if not os.path.isdir(d):
+            raise AmbError(f"{what}: directory {d} not found")
+        if not any(os.path.isfile(os.path.join(d, n)) for n in names):
+            raise AmbError(f"{what}: {os.path.join(d, names[0])} not found")
+
+
 class B200Module:
     config_class = None                                        # dataclass whose fields the constructor's **kwargs take
     weight_files = ("model.safetensors", "pytorch_model.bin")  # in order of preference

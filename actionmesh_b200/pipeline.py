@@ -1,18 +1,19 @@
-"""ActionMeshB200Pipeline / Stage1Pipeline / AnimationPipeline — the hot path of `ActionMeshPipeline.__call__` (reference actionmesh/pipeline.py:602-685) without the
-out-of-scope stages: DinoV2 context for all frames (`encode_all_frames`, :232-245), then the autoregressive Stage-I
-denoising over 16-frame windows (`generate_3d_latents` :435-508 -> `_denoise_latents` :247-314).
-
-Stage 0 (TripoSG anchor latent + mesh), background removal, IO and rendering stay on the reference (SURVEY 2.1 marks
-them out of scope); the anchor latent therefore comes in through a seeded `LatentBank`, exactly the object
-`init_banks_from_anchor` hands to `generate_3d_latents` in the reference (:661,:672).  `AnimationPipeline` adds Stage II
-(`generate_mesh_animation` :510-600 -> `_decode_displacement` :316-385) on the CUDA autoencoder: the anchor mesh comes in
-as vertex features (positions + unit normals, mesh_processor.py:85-101) and the result is a `VertexBank` (all output
-meshes share the anchor's faces, so only vertices are produced).
+"""ActionMeshB200Pipeline / Stage1Pipeline / AnimationPipeline — `ActionMeshPipeline.__call__` (reference
+actionmesh/pipeline.py:602-685) on the CUDA path.  `Stage1Pipeline` is DinoV2 context for all frames (`encode_all_frames`,
+:232-245), then the autoregressive Stage-I denoising over 16-frame windows (`generate_3d_latents` :435-508 ->
+`_denoise_latents` :247-314), from the anchor latent in a seeded `LatentBank`, exactly the object `init_banks_from_anchor`
+hands to `generate_3d_latents` in the reference (:661,:672).  `AnimationPipeline` adds Stage II (`generate_mesh_animation`
+:510-600 -> `_decode_displacement` :316-385) on the CUDA autoencoder: the anchor mesh comes in as vertex features
+(positions + unit normals, mesh_processor.py:85-101) and the result is a `VertexBank` (all output meshes share the anchor's
+faces, so only vertices are produced).
 
 `ActionMeshB200Pipeline` is seam 4 (SURVEY 8(b)): the reference's constructor and `__call__(input, seed, stage_0_steps,
 face_decimation, floaters_threshold, stage_1_steps, guidance_scales, anchor_idx) -> list of meshes` (pipeline.py:47-53,
-602-613) built from `actionmesh_b200*.yaml` through the same `_target_` plumbing, with the out-of-scope stages (TripoSG,
-background removal, CPU cropping, mesh post-processing) as injected components.
+602-613) built from `actionmesh_b200*.yaml` through the same `_target_` plumbing.  `ActionMeshB200Pipeline.from_pretrained(
+"pretrained_weights")` builds every stage from the reference's checkpoint directories: background removal
+(background_removal.py), cropping (preprocess.py), Stage 0 (stage0.py, triposg_vae.py), mesh post-processing
+(mesh_process.py), DinoV2, Stage I and Stage II.  The constructor instead takes the first three as injected components.
+IO and rendering stay on the reference.
 """
 from __future__ import annotations
 
@@ -258,9 +259,12 @@ class ActionMeshB200Pipeline:
     Built from `actionmesh_b200.yaml` / `actionmesh_b200_fast.yaml` (the reference's YAML with the `_target_`s re-pointed):
     scheduler, guidance, mesh post-process are instantiated at construction like the reference (:98-110); denoiser, image
     encoder and autoencoder are resolved from their `_target_`s and loaded from `weights_dir` by `.to()` (or assigned
-    directly — `pipe.temporal_3D_denoiser = model` — when weights do not come from disk).  Injected, because out of scope:
-      image_to_3d(image=, generator=, num_inference_steps=, guidance_scale=) -> (anchor_latent, anchor_mesh)   [TripoSG]
-      background_removal.process_images(frames), image_process.process_images(frames)                          [CPU, optional]
+    directly — `pipe.temporal_3D_denoiser = model` — when weights do not come from disk).
+
+    `from_pretrained(weights_root)` builds the whole pipeline from the reference's checkpoint layout.  The constructor
+    takes these components as injected arguments instead (any object with the same surface):
+      image_to_3d(image=, generator=, num_inference_steps=, guidance_scale=) -> (anchor_latent, anchor_mesh)   [TripoSGStage0]
+      background_removal.process_images(frames), image_process.process_images(frames)                          [optional]
     `anchor_mesh` needs `.vertices`, `.faces` and `.vertex_normals` (the trimesh attributes the reference reads)."""
 
     def __init__(self, config_name: str = "actionmesh_b200.yaml", config_dir: Optional[str] = None,
@@ -282,9 +286,77 @@ class ActionMeshB200Pipeline:
         self._target_device = torch.device("cpu")
         self._dtype = dtype            # accepted for signature compatibility: the CUDA path owns its precision recipe
         self._lazy_loading = lazy_loading
+        self._loaders: dict = {}       # attribute -> callable building it from a checkpoint (set by from_pretrained)
+
+    # ---- checkpoints (pipeline.py:66-83): the reference's four directories under `pretrained_weights/`
+    @classmethod
+    def _required_files(cls) -> list:
+        """(subdirectory of the weights root, file names of which one must exist) for every model this pipeline loads."""
+        from .background_removal import B200BackgroundRemover
+        from .stage0 import TRIPOSG_FILES
+
+        return ([(os.path.join("TripoSG", d), names) for d, names in TRIPOSG_FILES]
+                + [("dinov2", ("config.json",)), ("dinov2", B200ImageEncoder.weight_files),
+                   ("dinov2", ("preprocessor_config.json",)), ("RMBG", B200BackgroundRemover.weight_files)]
+                + [(os.path.join("ActionMesh", d), names) for d in ("denoiser", "autoencoder")
+                   for names in (("config.json",), B200Denoiser.weight_files)])
+
+    @classmethod
+    def from_pretrained(cls, weights_root: str = "pretrained_weights", config_name: str = "actionmesh_b200.yaml",
+                        config_dir: Optional[str] = None, lazy_loading: bool = False, *, dtype: torch.dtype = torch.bfloat16,
+                        config_updates: Optional[dict] = None):
+        """The pipeline the reference builds, from the reference's checkpoint directories under `weights_root`: TripoSG
+        (Stage 0), dinov2 (Stage I's image encoder, fp32-grade), RMBG (background removal) and ActionMesh (denoiser/,
+        autoencoder/).  Frames are cropped by `B200FramePreprocessor` and the anchor mesh is post-processed by
+        `B200MeshPostprocessor`.  Every required file is checked here, before any GPU work: a missing one raises an
+        AmbError naming it.  Models are loaded by `.to(device)`, or with `lazy_loading` just before their stage and
+        released right after it."""
+        from .mesh_process import B200MeshPostprocessor
+        from .module import check_files
+        from .preprocess import B200FramePreprocessor
+
+        check_files(weights_root, cls._required_files(), "ActionMesh checkpoints")
+        target = f"{B200MeshPostprocessor.__module__}.{B200MeshPostprocessor.__name__}"
+        pipe = cls(config_name, config_dir, dtype, lazy_loading, image_process=B200FramePreprocessor(),
+                   weights_dir=os.path.join(weights_root, "ActionMesh"),
+                   config_updates={"model.mesh_process._target_": target, **(config_updates or {})})
+        pipe._bind_checkpoints(weights_root)
+        return pipe
+
+    def _bind_checkpoints(self, weights_root: str) -> None:
+        """Loaders (callables, so that lazy loading never holds two large models at once) of the models that do not come
+        from the ActionMesh directory."""
+        from .background_removal import B200BackgroundRemover
+        from .stage0 import TripoSGStage0
+
+        dino = os.path.join(weights_root, "dinov2")
+        self._loaders = {
+            "background_removal": lambda: B200BackgroundRemover(os.path.join(weights_root, "RMBG")).to(self._target_device),
+            "image_to_3d_pipe": lambda: TripoSGStage0.from_pretrained(os.path.join(weights_root, "TripoSG"),
+                                                                      device=self._target_device,
+                                                                      num_tokens=self._denoiser_latent_shape[0]),
+            "image_encoder": lambda: B200ImageEncoder.from_hf_dirs(dino, dino, precision="fp32", device=self._target_device),
+        }
 
     # ---- model lifecycle (pipeline.py:117-229)
+    def _load_from_checkpoint(self, attr: str) -> None:
+        """Build `attr` with its checkpoint loader when it is not loaded; an injected component is left as it is."""
+        if getattr(self, attr) is None and attr in self._loaders:
+            setattr(self, attr, self._loaders[attr]())
+
+    def _release(self, attr: str) -> None:
+        """`_unload_model` for a component `from_pretrained` can load again (an injected one is kept)."""
+        if attr in self._loaders:
+            self._unload_model(attr)
+
+    def _load_image_to_3d(self) -> None:
+        self._load_from_checkpoint("image_to_3d_pipe")
+
+    def _load_background_removal(self) -> None:
+        self._load_from_checkpoint("background_removal")
+
     def _load_image_encoder(self) -> None:
+        self._load_from_checkpoint("image_encoder")
         if self.image_encoder is None:
             self.image_encoder = instantiate(self.cfg.model.image_encoder, _convert_="partial")()
         self.image_encoder.to(self._target_device)
@@ -314,6 +386,8 @@ class ActionMeshB200Pipeline:
             raise AmbError("ActionMeshB200Pipeline runs on CUDA (sm_90a) only; there is no CPU fallback")
         self._target_device = device
         if not self._lazy_loading:
+            self._load_background_removal()
+            self._load_image_to_3d()
             self._load_image_encoder()
             self._load_temporal_denoiser()
             self._load_temporal_vae()
@@ -340,16 +414,18 @@ class ActionMeshB200Pipeline:
             self.mesh_process.floaters_threshold = floaters_threshold
         if anchor_idx is not None:
             self.cfg.anchor_idx = anchor_idx
+        self._load_background_removal()
         if self.background_removal is not None:
             input.frames = self.background_removal.process_images(input.frames)
+        self._release("background_removal")
         if self.image_process is not None:
             input.frames = self.image_process.process_images(input.frames)
 
     def init_banks_from_anchor(self, input, seed: int = 44):
         """Stage 0 through the injected image-to-3D component (pipeline.py:387-433) -> (LatentBank, anchor mesh)."""
         if self.image_to_3d_pipe is None:
-            raise AmbError("Stage 0 (TripoSG image-to-3D) is not part of actionmesh_b200: pass image_to_3d=<callable> "
-                           "returning (anchor_latent, anchor_mesh)")
+            raise AmbError("no Stage 0 (TripoSG image-to-3D): build the pipeline with from_pretrained(weights_root) or pass "
+                           "image_to_3d=<callable> returning (anchor_latent, anchor_mesh)")
         gen_dev = getattr(self.image_to_3d_pipe, "device", self._target_device)
         anchor_latent, anchor_mesh = self.image_to_3d_pipe(
             image=input.frames[self.cfg.anchor_idx], generator=torch.Generator(device=gen_dev).manual_seed(seed),
@@ -380,7 +456,9 @@ class ActionMeshB200Pipeline:
         """video -> 4D (pipeline.py:602-685): returns the animated meshes (fixed topology) ordered by timestep."""
         self._apply_overrides(input, stage_0_steps, face_decimation, floaters_threshold, stage_1_steps, guidance_scales,
                               anchor_idx)
+        self._load_image_to_3d()
         latent_bank, anchor_mesh = self.init_banks_from_anchor(input, seed)          # Stage 0
+        self._release("image_to_3d_pipe")
         ordered = self._animate(input, latent_bank, anchor_mesh.vertices, anchor_mesh.faces, anchor_mesh.vertex_normals, seed)
         f_np = torch.as_tensor(anchor_mesh.faces).to(torch.int64).numpy()
         return [_make_output_mesh(v.cpu().numpy(), f_np) for v in ordered]
@@ -435,6 +513,20 @@ class ActionMeshB200PipelineWithMeshInput(ActionMeshB200Pipeline):
         super().__init__(*args, **kwargs)
         self._triposg_weights_dir = triposg_weights_dir
         self.vae = None
+
+    @classmethod
+    def _required_files(cls) -> list:
+        """The base pipeline's files, with TripoSG's VAE in place of the whole of Stage 0."""
+        from .triposg_vae import B200TripoSGVAE
+
+        vae = os.path.join("TripoSG", "vae")
+        return ([(vae, ("config.json",)), (vae, B200TripoSGVAE.weight_files)]
+                + [e for e in super()._required_files() if not e[0].startswith("TripoSG")])
+
+    def _bind_checkpoints(self, weights_root: str) -> None:
+        super()._bind_checkpoints(weights_root)
+        del self._loaders["image_to_3d_pipe"]
+        self._triposg_weights_dir = os.path.join(weights_root, "TripoSG")
 
     def _load_vae(self) -> None:
         if self.vae is None:

@@ -15,10 +15,13 @@ accumulation and an fp32 residual stream, latents stay fp32 between steps (the r
 scheduling_rectified_flow.py:299).  tests/test_stage0_gpu.py states the tolerance against the fp32 reference modules.
 The VAE decoder and the iso-surface extraction that turn the latent into the anchor MESH live in triposg_vae.py:
 `TripoSGStage0(..., mesh_extractor=B200TripoSGVAE.extract_mesh)` (bound to a loaded VAE).  Without an extractor,
-`__call__` raises.
+`__call__` raises.  `TripoSGStage0.from_pretrained(triposg_dir)` builds the DiT, the VAE, TripoSG's DinoV2 and the
+scheduler shift from the reference's TripoSG checkpoint directory (DESIGN section 18).
 """
 from __future__ import annotations
 
+import json
+import os
 from typing import Callable, Optional
 
 import numpy as np
@@ -28,7 +31,10 @@ from ._lib import AmbError
 from .blocks import remap_triposg_state_dict
 from .denoiser import B200Denoiser, DenoiserConfig
 from .guidance import ClassifierFreeGuidance
+from .image_encoder import B200ImageEncoder
+from .module import check_files
 from .scheduler import B200SchedulerFlow
+from .triposg_vae import B200TripoSGVAE
 
 
 class B200TripoSGDiT(B200Denoiser):
@@ -114,17 +120,57 @@ class _Stage0Flow(B200SchedulerFlow):
         return torch.cat([rf.timesteps, torch.zeros(1)]), rf.sigmas[:-1] - rf.sigmas[1:]
 
 
+def scheduler_shift(scheduler_dir: str) -> float:
+    """The `shift` of a diffusers `RectifiedFlowScheduler` directory (scheduler_config.json)."""
+    path = os.path.join(scheduler_dir, "scheduler_config.json")
+    if not os.path.isfile(path):
+        raise AmbError(f"TripoSG scheduler: {path} not found")
+    with open(path) as f:
+        cfg = json.load(f)
+    if cfg.get("use_dynamic_shifting", False):
+        raise AmbError("dynamic shifting is not used by ActionMesh's Stage 0")
+    if int(cfg.get("num_train_timesteps", 1000)) != 1000:
+        raise AmbError(f"TripoSG scheduler: num_train_timesteps {cfg['num_train_timesteps']} (expected 1000)")
+    return float(cfg.get("shift", 1.0))
+
+
+# Subfolders of the TripoSG checkpoint (diffusers layout) and the files each one must hold (one of each tuple).
+TRIPOSG_FILES = (("transformer", ("config.json",)), ("transformer", B200TripoSGDiT.weight_files),
+                 ("vae", ("config.json",)), ("vae", B200TripoSGVAE.weight_files),
+                 ("image_encoder_dinov2", ("config.json",)), ("image_encoder_dinov2", B200ImageEncoder.weight_files),
+                 ("feature_extractor_dinov2", ("preprocessor_config.json",)), ("scheduler", ("scheduler_config.json",)))
+
+
 class TripoSGStage0:
     """`image_to_3d` component of ActionMeshB200Pipeline: (image, generator, num_inference_steps, guidance_scale) ->
     (anchor_latent (1, N, C) fp32, anchor_mesh), as `TripoSGPipelinePlus.__call__` (actionmesh/external/triposg.py:35).
 
     `image_encoder`: B200ImageEncoder with TripoSG's DinoV2 weights (pipeline_triposg.py:137-145); `mesh_extractor(latents)`:
-    the VAE decode + iso-surface extraction, e.g. `B200TripoSGVAE(...).extract_mesh` (triposg_vae.py)."""
+    the VAE decode + iso-surface extraction, e.g. `B200TripoSGVAE(...).extract_mesh` (triposg_vae.py).
+    `from_pretrained(triposg_dir)` builds all of it from the TripoSG checkpoint directory."""
 
     def __init__(self, transformer: B200TripoSGDiT, image_encoder, mesh_extractor: Optional[Callable] = None,
                  shift: float = 1.0, num_tokens: int = 2048):
         self.transformer, self.image_encoder, self.mesh_extractor = transformer, image_encoder, mesh_extractor
         self.shift, self.num_tokens = shift, num_tokens
+
+    @classmethod
+    def from_pretrained(cls, triposg_dir: str, device="cuda", num_tokens: int = 2048) -> "TripoSGStage0":
+        """The TripoSG checkpoint directory (diffusers layout: transformer/, vae/, image_encoder_dinov2/,
+        feature_extractor_dinov2/, scheduler/) -> Stage 0 on `device`, with the VAE's `extract_mesh` at the defaults of
+        `TripoSGPipelinePlus.__call__` (bounds +-1.005, octree depth 9) as the mesh extractor.
+
+        TripoSG's DinoV2 runs with bf16 operands: the reference casts the whole TripoSG pipeline to fp16, and this package
+        uses bf16 where the reference uses fp16 in Stage 0 (DESIGN section 11).  bf16 also puts its attention on the wgmma
+        flash-attention kernel, which takes any sequence length, whatever crop the feature extractor asks for."""
+        check_files(triposg_dir, TRIPOSG_FILES, "TripoSG checkpoint")
+        shift = scheduler_shift(os.path.join(triposg_dir, "scheduler"))
+        transformer = B200TripoSGDiT.from_pretrained(os.path.join(triposg_dir, "transformer"), device=device)
+        vae = B200TripoSGVAE.from_pretrained(os.path.join(triposg_dir, "vae"), device=device)
+        encoder = B200ImageEncoder.from_hf_dirs(os.path.join(triposg_dir, "image_encoder_dinov2"),
+                                                os.path.join(triposg_dir, "feature_extractor_dinov2"), precision="bf16",
+                                                device=device)
+        return cls(transformer, encoder, mesh_extractor=vae.extract_mesh, shift=shift, num_tokens=num_tokens)
 
     @property
     def device(self) -> torch.device:
@@ -153,6 +199,6 @@ class TripoSGStage0:
                                   device=generator.device if generator is not None else self.device)
         lat = self.denoise(embeds.reshape(1, -1, embeds.shape[-1]), latents, num_inference_steps, guidance_scale)
         if self.mesh_extractor is None:
-            raise AmbError("TripoSGStage0: the VAE decoder / iso-surface extraction is not part of actionmesh_b200 — pass "
-                           "mesh_extractor=<callable latents -> mesh>")
+            raise AmbError("TripoSGStage0: no mesh extractor — pass mesh_extractor=<callable latents -> mesh> (e.g. "
+                           "B200TripoSGVAE.extract_mesh) or build it with TripoSGStage0.from_pretrained")
         return lat, self.mesh_extractor(lat)
