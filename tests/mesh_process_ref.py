@@ -226,30 +226,43 @@ def drop_unreferenced(pos, faces):
     return pos[used], remap[faces]
 
 
+def one_round(pos, q, faces, target: int, adj: Adjacency | None = None):
+    """One decimation round of a mesh with more than `target` faces -> (positions, quadrics, faces) after it, or None when
+    no valid collapse is left.  The inputs are not modified; `adj` is Adjacency(faces, len(pos)) when the caller has it."""
+    V = len(pos)
+    if adj is None:
+        adj = Adjacency(faces, V)
+    keys, targets, m2 = select(pos, q, faces, adj)
+    win = (keys != NO_KEY) & (keys == m2[adj.a]) & (keys == m2[adj.b])
+    if not win.any():
+        return None
+    limit, removed = round_limit(keys[win], adj.nf[win], len(faces), target)
+    w = np.flatnonzero(win & (keys <= limit))
+    a, b = adj.a[w], adj.b[w]
+    remap = np.arange(V)
+    remap[b] = a
+    pos, q = pos.copy(), q.copy()
+    pos[a] = targets[w]
+    q[a] = q[a] + q[b]
+    faces = remap[faces]
+    faces = faces[(faces[:, 0] != faces[:, 1]) & (faces[:, 1] != faces[:, 2]) & (faces[:, 0] != faces[:, 2])]
+    return pos, q, faces
+
+
 def decimate(vertices: np.ndarray, faces: np.ndarray, target: int):
     """-> (vertices (V', 3) float64, faces (F', 3) int64, rounds); the input must be clean (mesh_input.clean_topology)."""
     pos = np.array(vertices, dtype=np.float64)
     faces = np.asarray(faces, dtype=np.int64)
-    V = len(pos)
     q = None
     rounds = 0
     while len(faces) > target:
-        adj = Adjacency(faces, V)
+        adj = Adjacency(faces, len(pos))
         if q is None:
             q = quadrics(pos, faces, adj)
-        keys, targets, m2 = select(pos, q, faces, adj)
-        win = (keys != NO_KEY) & (keys == m2[adj.a]) & (keys == m2[adj.b])
-        if not win.any():
+        state = one_round(pos, q, faces, target, adj)
+        if state is None:
             break
-        limit, removed = round_limit(keys[win], adj.nf[win], len(faces), target)
-        w = np.flatnonzero(win & (keys <= limit))
-        a, b = adj.a[w], adj.b[w]
-        remap = np.arange(V)
-        remap[b] = a
-        pos[a] = targets[w]
-        q[a] = q[a] + q[b]
-        faces = remap[faces]
-        faces = faces[(faces[:, 0] != faces[:, 1]) & (faces[:, 1] != faces[:, 2]) & (faces[:, 0] != faces[:, 2])]
+        pos, q, faces = state
         rounds += 1
     pos, faces = drop_unreferenced(pos, faces)
     return pos, faces, rounds
@@ -356,6 +369,30 @@ def floater_mesh():
     v, f = clean_topology(v, f)                        # merges the shared cube corner into one vertex
     perm = np.random.default_rng(0).permutation(len(f))
     return v, f[perm]
+
+
+def blob_field(n_blobs: int = 40, seed: int = 0):
+    """A multi-component test field for triposg_vae_ref.dense_grid: xyz (P, 3) fp32 torch -> (P, 1) logits, positive inside.
+    A sum of seeded Gaussian blobs around two cluster centres, which mesh to two large components, plus one small isolated
+    blob whose component is far below 2 % of the largest one's faces."""
+    import torch
+
+    rng = np.random.default_rng(seed)
+    hub = np.where(np.arange(n_blobs)[:, None] % 3 == 2, [0.5, 0.1, 0.0], [-0.5, -0.1, 0.0])
+    centres = np.concatenate([hub + rng.uniform(-0.28, 0.28, (n_blobs, 3)), [[0.0, -0.7, 0.7]]])
+    radii = np.concatenate([rng.uniform(0.1, 0.2, n_blobs), [0.045]])
+    c = torch.from_numpy(centres.astype(np.float32))
+    inv = torch.from_numpy((1.0 / (radii * radii)).astype(np.float32))
+
+    def field(xyz):
+        cd, invd = c.to(xyz.device), inv.to(xyz.device)
+        out = []
+        for p in xyz.split(1 << 18):
+            d2 = ((p[:, None, :] - cd[None]) ** 2).sum(-1)
+            out.append((torch.exp(-d2 * invd).sum(-1, keepdim=True) - 0.5) * 8.0)
+        return torch.cat(out)
+
+    return field
 
 
 def soup_mesh(V: int = 200, F: int = 600, seed: int = 3):
