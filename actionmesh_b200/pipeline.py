@@ -13,7 +13,8 @@ face_decimation, floaters_threshold, stage_1_steps, guidance_scales, anchor_idx)
 "pretrained_weights")` builds every stage from the reference's checkpoint directories: background removal
 (background_removal.py), cropping (preprocess.py), Stage 0 (stage0.py, triposg_vae.py), mesh post-processing
 (mesh_process.py), DinoV2, Stage I and Stage II.  The constructor instead takes the first three as injected components.
-IO and rendering stay on the reference.
+Frames are read by video_input.py, meshes read and written by gltf.py, rendered by render.py, and inference.py is the
+command line that ties them to the pipeline.
 """
 from __future__ import annotations
 
@@ -224,9 +225,11 @@ class PassThroughMeshProcess:
 
 @dataclass
 class Mesh:
-    """Minimal mesh record returned when `trimesh` is not installed: (V, 3) float32 vertices + (F, 3) int faces (numpy)."""
+    """Minimal mesh record returned when `trimesh` is not installed: (V, 3) float32 vertices + (F, 3) int faces (numpy).
+    `visual` is the texture side `gltf.load_glb` reads (a `gltf.GltfVisual`), or None."""
     vertices: "object"
     faces: "object"
+    visual: "object" = None
 
 
 def _vertex_normals(vertices: torch.Tensor, faces: torch.Tensor) -> torch.Tensor:

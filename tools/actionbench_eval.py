@@ -18,23 +18,15 @@ import argparse
 import csv
 import json
 import math
-import os
-import re
 import sys
 from pathlib import Path
 
 import numpy as np
 
+sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
+from actionmesh_b200.video_input import natural_sorted  # noqa: E402  (meshes sort in the order frames load)
+
 COLUMNS = ["uid", "cd_3d", "cd_4d", "cd_motion", "n_frames", "status", "error_message"]
-
-
-def natural_sorted(names) -> list:
-    """Sort by the digit runs of each name as numbers and the rest as lower-case text (natsort's default order on these
-    file names)."""
-    def key(name):
-        parts = re.split(r"(\d+)", os.path.basename(str(name)))
-        return [(0, int(p), "") if p.isdigit() else (1, 0, p.lower()) for p in parts if p != ""]
-    return sorted(names, key=key)
 
 
 def find_uids(gt_root: Path, pred_root: Path, mesh_pattern: str = "mesh_*.glb") -> list[str]:
@@ -164,7 +156,6 @@ def main() -> None:
     ap.add_argument("--recompute", action="store_true")
     ap.add_argument("--no_4d", action="store_true", help="skip the motion Chamfer distance (cd_motion = 0)")
     a = ap.parse_args()
-    sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
     rows = evaluate_dataset(a.gt_root, a.pred_root, a.output_csv, mesh_pattern=a.mesh_pattern, recompute=a.recompute,
                             device=a.device, n_pts_icp=a.n_pts_icp, n_pts_chamfer=a.n_pts_chamfer, seed=a.seed,
                             is_4d=not a.no_4d)
