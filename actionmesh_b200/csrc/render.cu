@@ -244,10 +244,199 @@ __global__ void shade_kernel(const float* __restrict__ verts, const int32_t* __r
   }
 }
 
+// ---- texture shading -------------------------------------------------------------------------------------------------------
+
+constexpr int kMaxTexSide = 16384;
+constexpr int kMaxLevels = 15;  // 16384 -> 1 in 14 halvings
+constexpr float kUvLimit = 32768.0f;
+
+enum : int {
+  kNearest = 9728,
+  kLinear = 9729,
+  kNearestMipNearest = 9984,
+  kLinearMipNearest = 9985,
+  kNearestMipLinear = 9986,
+  kLinearMipLinear = 9987,
+  kRepeat = 10497,
+  kClampToEdge = 33071,
+  kMirroredRepeat = 33648,
+};
+
+// the mip chain as a kernel parameter: level l is h[l] rows of w[l] RGB texels at byte offset off[l] of the level buffer
+struct TexLevels {
+  long long off[kMaxLevels];
+  int w[kMaxLevels], h[kMaxLevels];
+  int n;
+};
+
+struct Sampler {
+  int mag, min, wrap_s, wrap_t;
+  float base[3];
+};
+
+// level l + 1 texel (x, y) = floor((a + b + c + d + 2) / 4) per channel over level-l texels (min(2x+dx, w-1), min(2y+dy, h-1))
+__global__ void texture_level_kernel(uint8_t* __restrict__ levels, long long src_off, int sw, int sh, long long dst_off,
+                                     int dw, int dh) {
+  const long long n = (long long)dw * dh;
+  const uint8_t* src = levels + src_off;
+  uint8_t* dst = levels + dst_off;
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < n; p += (long long)gridDim.x * blockDim.x) {
+    const int x = (int)(p % dw), y = (int)(p / dw);
+    const int x0 = min(2 * x, sw - 1), x1 = min(2 * x + 1, sw - 1), y0 = min(2 * y, sh - 1), y1 = min(2 * y + 1, sh - 1);
+    const uint8_t* r0 = src + 3LL * y0 * sw;
+    const uint8_t* r1 = src + 3LL * y1 * sw;
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      dst[3 * p + k] = (uint8_t)((r0[3 * x0 + k] + r0[3 * x1 + k] + r1[3 * x0 + k] + r1[3 * x1 + k] + 2) >> 2);
+  }
+}
+
+__device__ __forceinline__ int wrap_index(int i, int n, int mode) {
+  if (mode == kClampToEdge) return clampi(i, 0, n - 1);
+  if (mode == kMirroredRepeat) {
+    const int m = ((i % (2 * n)) + 2 * n) % (2 * n);
+    return m < n ? m : 2 * n - 1 - m;
+  }
+  return ((i % n) + n) % n;  // REPEAT
+}
+
+// filtered RGB (0..255, not rounded) of level `l` at (u, v): NEAREST texel (floor(u w), floor(v h)), or LINEAR around
+// (u w - 1/2, v h - 1/2) with weights ((t00 (1-fx) + t10 fx) (1-fy)) + ((t01 (1-fx) + t11 fx) fy)
+__device__ __forceinline__ void sample_level(const uint8_t* __restrict__ levels, const TexLevels& tl, int l, bool linear,
+                                             int wrap_s, int wrap_t, float u, float v, float* rgb) {
+  const int w = tl.w[l], h = tl.h[l];
+  const uint8_t* base = levels + tl.off[l];
+  u = fminf(fmaxf(u, -kUvLimit), kUvLimit);
+  v = fminf(fmaxf(v, -kUvLimit), kUvLimit);
+  if (!linear) {
+    const int x = wrap_index((int)floorf(fm(u, (float)w)), w, wrap_s), y = wrap_index((int)floorf(fm(v, (float)h)), h, wrap_t);
+    const uint8_t* t = base + 3LL * ((long long)y * w + x);
+    rgb[0] = (float)t[0];
+    rgb[1] = (float)t[1];
+    rgb[2] = (float)t[2];
+    return;
+  }
+  const float x = fs(fm(u, (float)w), 0.5f), y = fs(fm(v, (float)h), 0.5f);
+  const float xf = floorf(x), yf = floorf(y);
+  const float fx = fs(x, xf), fy = fs(y, yf), gx = fs(1.0f, fx), gy = fs(1.0f, fy);
+  const int xi = (int)xf, yi = (int)yf;
+  const int xa = wrap_index(xi, w, wrap_s), xb = wrap_index(xi + 1, w, wrap_s);
+  const int ya = wrap_index(yi, h, wrap_t), yb = wrap_index(yi + 1, h, wrap_t);
+  const uint8_t* r0 = base + 3LL * ya * w;
+  const uint8_t* r1 = base + 3LL * yb * w;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float t00 = r0[3 * xa + k], t10 = r0[3 * xb + k], t01 = r1[3 * xa + k], t11 = r1[3 * xb + k];
+    rgb[k] = fa(fm(fa(fm(t00, gx), fm(t10, fx)), gy), fm(fa(fm(t01, gx), fm(t11, fx)), fy));
+  }
+}
+
+// the shaded colour of one sample covered by face f (DESIGN §16, texture shading)
+__device__ __forceinline__ void texture_sample(const float* __restrict__ verts, const int32_t* __restrict__ faces,
+                                               const float* __restrict__ normals, const float* __restrict__ uv,
+                                               const float* cp, float focal, int S, int f, int r, int c,
+                                               const uint8_t* __restrict__ levels, const TexLevels& tl,
+                                               const Sampler& sm, float* col) {
+  const int n2 = 2 * S;
+  const Face s = face_setup(verts, faces, f, cp, focal, n2);
+  Bary b;
+  barycentrics(s, sample_ndc(c, n2), sample_ndc(r, n2), &b);  // inside: pix_to_face came from this test
+  const int i0 = faces[3LL * f], i1 = faces[3LL * f + 1], i2 = faces[3LL * f + 2];
+  const P3 a0 = load3(normals, i0), a1 = load3(normals, i1), a2 = load3(normals, i2);
+  const P3 n = {fa(fa(fm(b.b0, a0.x), fm(b.b1, a1.x)), fm(b.b2, a2.x)), fa(fa(fm(b.b0, a0.y), fm(b.b1, a1.y)), fm(b.b2, a2.y)),
+                fa(fa(fm(b.b0, a0.z), fm(b.b1, a1.z)), fm(b.b2, a2.z))};
+  // n R (rotation only), normalised; two-sided headlight
+  const float vx = fa(fa(fm(n.x, cp[0]), fm(n.y, cp[3])), fm(n.z, cp[6]));
+  const float vy = fa(fa(fm(n.x, cp[1]), fm(n.y, cp[4])), fm(n.z, cp[7]));
+  const float vz = fa(fa(fm(n.x, cp[2]), fm(n.y, cp[5])), fm(n.z, cp[8]));
+  const float len = __fsqrt_rn(fa(fa(fm(vx, vx), fm(vy, vy)), fm(vz, vz)));
+  const float shade = fa(0.35f, fm(0.65f, fabsf(fd(vz, len > kShadeEps ? len : kShadeEps))));
+  float base[3] = {sm.base[0], sm.base[1], sm.base[2]};
+  if (tl.n) {
+    const float u0 = uv[2LL * i0], w0 = uv[2LL * i0 + 1], u1 = uv[2LL * i1], w1 = uv[2LL * i1 + 1];
+    const float u2 = uv[2LL * i2], w2 = uv[2LL * i2 + 1];
+    const float u = fa(fa(fm(b.b0, u0), fm(b.b1, u1)), fm(b.b2, u2)), v = fa(fa(fm(b.b0, w0), fm(b.b1, w1)), fm(b.b2, w2));
+    // level of detail of (face, view): projected area A_s in samples against the uv area A_t in level-0 texels
+    const float a_s = fm(fm(0.5f, fabsf(edge(s.v0.x, s.v0.y, s.v1, s.v2))), (float)(S * S));
+    const float a_t = fm(fm(0.5f, fabsf(fs(fm(fs(u0, u1), fs(w2, w1)), fm(fs(w0, w1), fs(u2, u1))))),
+                         (float)((long long)tl.w[0] * tl.h[0]));
+    int level = 0, filter = sm.mag;  // magnified, or a face with a depth <= 0
+    if (s.v0.z > 0.0f && s.v1.z > 0.0f && s.v2.z > 0.0f && !(a_t <= a_s)) {
+      filter = sm.min;
+      if (sm.min >= kNearestMipNearest) {
+        float lim = a_s;
+        while (level < tl.n - 1 && !(a_t <= lim)) {
+          lim = fm(lim, 4.0f);
+          ++level;
+        }
+      }
+    }
+    const bool linear = filter == kLinear || filter == kLinearMipNearest || filter == kLinearMipLinear;
+    float t[3];
+    sample_level(levels, tl, level, linear, sm.wrap_s, sm.wrap_t, u, v, t);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) base[k] = fm(base[k], fd(t[k], 255.0f));
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) col[k] = fm(base[k], shade);
+}
+
+// one thread per output pixel (view, i, j): the mean of its four samples' shaded colours (white where no face), truncated
+__global__ void __launch_bounds__(256) shade_texture_kernel(const float* __restrict__ verts, const int32_t* __restrict__ faces,
+                                                            const float* __restrict__ normals, const float* __restrict__ uv,
+                                                            const float* __restrict__ cams, int n_cams, float focal, int S,
+                                                            const int32_t* __restrict__ pix_to_face,
+                                                            const uint8_t* __restrict__ levels, const TexLevels tl,
+                                                            const Sampler sm, uint8_t* __restrict__ out,
+                                                            long long row_stride, int view_stride) {
+  const int n2 = 2 * S;
+  const long long n = (long long)n_cams * S * S;
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < n; p += (long long)gridDim.x * blockDim.x) {
+    const int cam = (int)(p / ((long long)S * S)), i = (int)(p / S % S), j = (int)(p % S);
+    const float* cp = cams + 12 * cam;
+    const int32_t* pf = pix_to_face + (long long)cam * n2 * n2;
+    float acc[3];
+#pragma unroll 1
+    for (int q = 0; q < 4; ++q) {
+      const int r = 2 * i + (q >> 1), c = 2 * j + (q & 1);
+      const int f = pf[(long long)r * n2 + c];
+      float col[3] = {1.0f, 1.0f, 1.0f};
+      if (f >= 0) texture_sample(verts, faces, normals, uv, cp, focal, S, f, r, c, levels, tl, sm, col);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) acc[k] = q ? fa(acc[k], col[k]) : col[k];
+    }
+    uint8_t* o = out + (long long)i * row_stride + (long long)cam * view_stride + 3LL * j;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) o[k] = (uint8_t)(int)fm(fminf(fmaxf(fm(acc[k], 0.25f), 0.0f), 1.0f), 255.0f);
+  }
+}
+
 constexpr int kThreads = 256;
 
 bool render_sizes_ok(int64_t n_vertices, int64_t n_faces) {
   return n_vertices >= 0 && n_faces >= 0 && n_vertices < (1LL << 31) - 1 && 6 * n_faces < (1LL << 31);
+}
+
+// a full mip chain: level 0 of 1..16384 texels a side, each next level halved (at least 1), down to 1 x 1, in ascending
+// non-overlapping byte ranges; false with the reason in *why
+bool level_table_ok(const int64_t* table, int n_levels, TexLevels* tl, const char** why) {
+  *why = "";
+  if (n_levels < 1 || n_levels > kMaxLevels) return *why = "n_levels outside [1, 15]", false;
+  long long end = 0;
+  for (int l = 0; l < n_levels; ++l) {
+    const int64_t off = table[3 * l], w = table[3 * l + 1], h = table[3 * l + 2];
+    if (l == 0 && (w < 1 || h < 1 || w > kMaxTexSide || h > kMaxTexSide)) return *why = "level 0 size outside [1, 16384]", false;
+    if (l > 0 && (w != (tl->w[l - 1] > 1 ? tl->w[l - 1] >> 1 : 1) || h != (tl->h[l - 1] > 1 ? tl->h[l - 1] >> 1 : 1)))
+      return *why = "a level is not the previous one halved", false;
+    if (off < end) return *why = "level byte ranges overlap or descend", false;
+    tl->off[l] = off;
+    tl->w[l] = (int)w;
+    tl->h[l] = (int)h;
+    end = off + 3 * w * h;
+  }
+  if (tl->w[n_levels - 1] != 1 || tl->h[n_levels - 1] != 1) return *why = "the chain does not end at 1 x 1", false;
+  tl->n = n_levels;
+  return true;
 }
 
 }  // namespace
@@ -317,6 +506,59 @@ int amb_render_shade_normals(const float* vertices, int64_t n_vertices, const in
   const long long n = (long long)n_cameras * image_size * image_size;
   shade_kernel<<<blocks_for(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
       vertices, faces, normals, cameras, n_cameras, focal, image_size, pix_to_face, out, row_stride, (int)view_stride);
+  AMB_CHECK_CUDA(cudaGetLastError());
+  return AMB_OK;
+}
+
+int amb_render_texture_levels(uint8_t* levels, const int64_t* level_table, int n_levels, amb_stream_t stream) {
+  AMB_CHECK_ARG(levels && level_table, "render_texture_levels: null pointer");
+  TexLevels tl;
+  const char* why;
+  AMB_CHECK_ARG(level_table_ok(level_table, n_levels, &tl, &why), "render_texture_levels: bad level table (%s)", why);
+  for (int l = 1; l < n_levels; ++l) {
+    texture_level_kernel<<<blocks_for((long long)tl.w[l] * tl.h[l], kThreads), kThreads, 0, (cudaStream_t)stream>>>(
+        levels, tl.off[l - 1], tl.w[l - 1], tl.h[l - 1], tl.off[l], tl.w[l], tl.h[l]);
+    AMB_CHECK_CUDA(cudaGetLastError());
+  }
+  return AMB_OK;
+}
+
+int amb_render_shade_texture(const float* vertices, int64_t n_vertices, const int32_t* faces, int64_t n_faces,
+                             const float* normals, const float* uv, const float* cameras, int n_cameras, float focal,
+                             int image_size, const int32_t* pix_to_face, const uint8_t* levels, const int64_t* level_table,
+                             int n_levels, int mag_filter, int min_filter, int wrap_s, int wrap_t, float base_r,
+                             float base_g, float base_b, uint8_t* out, int64_t row_stride, int64_t view_stride,
+                             amb_stream_t stream) {
+  AMB_CHECK_ARG((!n_faces || (vertices && faces && normals && (!n_levels || uv))) && (!n_levels || (levels && level_table)) &&
+                    cameras && pix_to_face && out,
+                "render_shade_texture: null pointer");
+  AMB_CHECK_ARG(render_sizes_ok(n_vertices, n_faces), "render_shade_texture: bad mesh size (%lld vertices, %lld faces)",
+                (long long)n_vertices, (long long)n_faces);
+  AMB_CHECK_ARG(n_cameras >= 1 && image_size >= 1,
+                "render_shade_texture: need n_cameras >= 1 and image_size >= 1 (got %d, %d)", n_cameras, image_size);
+  const long long n2 = 2LL * image_size;
+  AMB_CHECK_ARG((long long)n_cameras * n2 * n2 < (1LL << 31), "render_shade_texture: %d cameras x %lld samples overflow int32",
+                n_cameras, n2 * n2);
+  AMB_CHECK_ARG(row_stride >= 3LL * image_size && view_stride >= 0 && view_stride < (1LL << 31) &&
+                    (n_cameras == 1 || view_stride >= 3LL * image_size),
+                "render_shade_texture: bad strides (row %lld, view %lld)", (long long)row_stride, (long long)view_stride);
+  AMB_CHECK_ARG(mag_filter == kNearest || mag_filter == kLinear, "render_shade_texture: bad mag_filter %d", mag_filter);
+  AMB_CHECK_ARG(min_filter == kNearest || min_filter == kLinear || (min_filter >= kNearestMipNearest && min_filter <= kLinearMipLinear),
+                "render_shade_texture: bad min_filter %d", min_filter);
+  for (int wrap : {wrap_s, wrap_t})
+    AMB_CHECK_ARG(wrap == kRepeat || wrap == kClampToEdge || wrap == kMirroredRepeat, "render_shade_texture: bad wrap mode %d",
+                  wrap);
+  TexLevels tl;
+  tl.n = 0;
+  if (n_levels) {
+    const char* why;
+    AMB_CHECK_ARG(level_table_ok(level_table, n_levels, &tl, &why), "render_shade_texture: bad level table (%s)", why);
+  }
+  const Sampler sm = {mag_filter, min_filter, wrap_s, wrap_t, {base_r, base_g, base_b}};
+  const long long n = (long long)n_cameras * image_size * image_size;
+  shade_texture_kernel<<<blocks_for(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
+      vertices, faces, normals, uv, cameras, n_cameras, focal, image_size, pix_to_face, levels, tl, sm, out, row_stride,
+      (int)view_stride);
   AMB_CHECK_CUDA(cudaGetLastError());
   return AMB_OK;
 }

@@ -1,11 +1,13 @@
 """The command line: video (+ optional .glb mesh) -> animated meshes on disk, on this package alone.
 
     python -m actionmesh_b200.inference --input clip.mp4 [--mesh_input mesh.glb] [--output_dir DIR] [--fast] [--low_ram]
+                                        [--render_texture]
 
 One entry point for the reference's `inference/video_to_animated_mesh.py` and `inference/video_and_3d_to_animated_mesh.py`
 (`--mesh_input` selects the second), with their flags and defaults plus `--weights_root`.  It writes, in `--output_dir`
 (default outputs/<input stem>): mesh_00.glb ..., deformations_vertices.npy, deformations_faces.npy, animated_mesh.glb and
-grid_normal.mp4.  `--blender_path` and `--dtype` are accepted so that the reference's documented command lines run
+grid_normal.mp4, and with `--render_texture` also grid_texture.mp4 (the meshes shaded with the input mesh's texture, or
+with the default colour).  `--blender_path` and `--dtype` are accepted so that the reference's documented command lines run
 unchanged, and have no effect: the animated GLB is written without Blender, and the CUDA path owns its precision.
 """
 from __future__ import annotations
@@ -33,9 +35,10 @@ ANIMATION_FPS = 8
 
 @torch.no_grad()
 def run_actionmesh(pipeline, input: str, output_dir: str, seed: int = 44, mesh_input: Optional[str] = None,
-                   **overrides) -> list:
+                   render_texture: bool = False, **overrides) -> list:
     """The reference scripts' `run_actionmesh`: load the frames (and the mesh), run `pipeline`, write every output file
-    into `output_dir` -> the meshes.  `overrides` are the pipeline's per-call arguments (stage_0_steps, face_decimation,
+    into `output_dir` -> the meshes.  `render_texture` adds grid_texture.mp4, shaded with the input mesh's visual (the one
+    the animated GLB gets).  `overrides` are the pipeline's per-call arguments (stage_0_steps, face_decimation,
     floaters_threshold, stage_1_steps, guidance_scales, anchor_idx)."""
     frames = load_frames(input, max_frames=MAX_FRAMES)
     visual = None
@@ -55,7 +58,12 @@ def run_actionmesh(pipeline, input: str, output_dir: str, seed: int = 44, mesh_i
     write_animated_glb(animated, np.stack([np.asarray(m.vertices) for m in meshes]), faces, fps=ANIMATION_FPS,
                        visual=visual)
     logger.info(f"Animated GLB saved to {animated}")
-    render.B200MeshVisualizer(image_size=256).render(meshes, pipeline.device, output_dir, frames.frames)
+    visualizer = render.B200MeshVisualizer(image_size=256)
+    if render_texture:
+        visualizer.render(meshes, pipeline.device, output_dir, frames.frames, modalities=("normal", "texture"),
+                          visual=visual)
+    else:
+        visualizer.render(meshes, pipeline.device, output_dir, frames.frames)
     return meshes
 
 
@@ -79,6 +87,8 @@ def parse_args(argv=None) -> argparse.Namespace:
     p.add_argument("--stage_1_steps", type=int, default=None, help="Stage I denoising steps. Default: 30. Fast: 15")
     p.add_argument("--guidance_scales", type=float, nargs="+", default=None, help="Stage I CFG scales. Default: [7.5]")
     p.add_argument("--anchor_idx", type=int, default=None, help="Index of the anchor frame. Default: 0")
+    p.add_argument("--render_texture", action="store_true",
+                   help="Also write grid_texture.mp4: the meshes shaded with the input mesh's texture (or a flat colour).")
     return p.parse_args(argv)
 
 
@@ -95,7 +105,8 @@ def main(argv=None) -> list:
     pipeline = cls.from_pretrained(args.weights_root, config_name=config_name, lazy_loading=args.low_ram).to("cuda")
     overrides = {k: getattr(args, k) for k in ("stage_0_steps", "face_decimation", "floaters_threshold",
                                                "stage_1_steps", "guidance_scales", "anchor_idx")}
-    return run_actionmesh(pipeline, args.input, output_dir, seed=args.seed, mesh_input=args.mesh_input, **overrides)
+    return run_actionmesh(pipeline, args.input, output_dir, seed=args.seed, mesh_input=args.mesh_input,
+                          render_texture=args.render_texture, **overrides)
 
 
 if __name__ == "__main__":

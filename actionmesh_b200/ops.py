@@ -744,6 +744,76 @@ def shade_normals(vertices: torch.Tensor, faces: torch.Tensor, normals: torch.Te
     return out
 
 
+# glTF sampler enums (the C ABI takes them as they are)
+NEAREST, LINEAR = 9728, 9729
+NEAREST_MIPMAP_NEAREST, LINEAR_MIPMAP_NEAREST, NEAREST_MIPMAP_LINEAR, LINEAR_MIPMAP_LINEAR = 9984, 9985, 9986, 9987
+REPEAT, CLAMP_TO_EDGE, MIRRORED_REPEAT = 10497, 33071, 33648
+MAG_FILTERS = (NEAREST, LINEAR)
+MIN_FILTERS = (NEAREST, LINEAR, NEAREST_MIPMAP_NEAREST, LINEAR_MIPMAP_NEAREST, NEAREST_MIPMAP_LINEAR, LINEAR_MIPMAP_LINEAR)
+WRAP_MODES = (REPEAT, CLAMP_TO_EDGE, MIRRORED_REPEAT)
+
+
+def texture_level_table(width: int, height: int) -> list[tuple[int, int, int]]:
+    """(byte offset, width, height) of every level of the full mip chain of a width x height RGB texture, packed."""
+    table, off, w, h = [], 0, int(width), int(height)
+    while True:
+        table.append((off, w, h))
+        off += 3 * w * h
+        if w == 1 and h == 1:
+            return table
+        w, h = max(1, w >> 1), max(1, h >> 1)
+
+
+def texture_levels(image: torch.Tensor) -> tuple[torch.Tensor, list[tuple[int, int, int]]]:
+    """The mip chain of an (h, w, 3) uint8 CUDA image -> (levels, table): every level packed into one uint8 buffer at the
+    byte offsets of `texture_level_table`; level l + 1 averages 2 x 2 texels of level l, rounding half up."""
+    dev = _device(image, "image")
+    assert image.dim() == 3 and image.shape[2] == 3 and image.dtype == torch.uint8, "image: expected (h, w, 3) uint8"
+    h, w = image.shape[:2]
+    table = texture_level_table(w, h)
+    off, lw, lh = table[-1]
+    levels = torch.empty(off + 3 * lw * lh, dtype=torch.uint8, device=image.device)
+    levels[:3 * w * h].copy_(image.reshape(-1))
+    _launch(_abi.amb_render_texture_levels, len(table) - 1, _ptr(levels, torch.uint8, "levels", dev),
+            (C.c_int64 * (3 * len(table)))(*[x for row in table for x in row]), len(table))
+    return levels, table
+
+
+def shade_texture(vertices: torch.Tensor, faces: torch.Tensor, normals: torch.Tensor, cameras: torch.Tensor, focal: float,
+                  pix_to_face: torch.Tensor, uv: Optional[torch.Tensor] = None, levels: Optional[torch.Tensor] = None,
+                  table: Optional[list] = None, *, mag_filter: int = LINEAR, min_filter: int = LINEAR_MIPMAP_NEAREST,
+                  wrap_s: int = REPEAT, wrap_t: int = REPEAT, base_color=(1.0, 1.0, 1.0),
+                  out: Optional[torch.Tensor] = None, column: int = 0) -> torch.Tensor:
+    """The texture-shaded images of `rasterize`'s views as uint8 RGB: each output pixel the mean of its four samples' colour
+    base(uv) x (0.35 + 0.65 |n_view.z|), white where no face covers a sample.  `levels` / `table` come from
+    `texture_levels`, and `uv` (V, 2) fp32 places the vertices on it; without them the colour is `base_color` times the
+    headlight.  Same `out` / `column` layout as `shade_normals` -> out."""
+    dev, V, F = _render_mesh(vertices, faces)
+    n_cams = _cameras(cameras)
+    assert pix_to_face.dim() == 3 and pix_to_face.shape[0] == n_cams and pix_to_face.shape[1] == pix_to_face.shape[2] \
+        and pix_to_face.shape[1] % 2 == 0 and pix_to_face.is_contiguous(), "pix_to_face: expected a contiguous (C, 2S, 2S) tensor"
+    assert normals.shape == vertices.shape and normals.is_contiguous(), "normals: expected a contiguous (V, 3) tensor"
+    assert (levels is None) == (table is None), "levels and table go together"
+    if levels is not None:
+        assert uv is not None and tuple(uv.shape) == (V, 2) and uv.is_contiguous(), "uv: expected a contiguous (V, 2) tensor"
+    S = pix_to_face.shape[1] // 2
+    if out is None:
+        out = torch.empty(S, n_cams * S, 3, dtype=torch.uint8, device=vertices.device)
+    assert out.dim() == 3 and out.shape[0] == S and out.shape[2] == 3 and out.stride(2) == 1 and out.stride(1) == 3 \
+        and 0 <= column and (column + n_cams) * S <= out.shape[1], "out: expected an (S, >= (column + C) * S, 3) row-major tensor"
+    cells = out[:, column * S:(column + n_cams) * S]
+    n_levels = 0 if table is None else len(table)
+    table_arg = None if table is None else (C.c_int64 * (3 * n_levels))(*[x for row in table for x in row])
+    r, g, b = (float(x) for x in base_color)
+    _launch(_abi.amb_render_shade_texture, 1, _ptr(vertices, torch.float32, "vertices", dev), V,
+            _ptr(faces, torch.int32, "faces", dev), F, _ptr(normals, torch.float32, "normals", dev),
+            _ptr(uv if levels is not None else None, torch.float32, "uv", dev), _ptr(cameras, torch.float32, "cameras", dev),
+            n_cams, float(focal), S, _ptr(pix_to_face, torch.int32, "pix_to_face", dev),
+            _ptr(levels, torch.uint8, "levels", dev), table_arg, n_levels, int(mag_filter), int(min_filter), int(wrap_s),
+            int(wrap_t), r, g, b, _ptr(cells, torch.uint8, "out", dev), out.stride(0), 3 * S)
+    return out
+
+
 def _icp_tensor(t: torch.Tensor, shape: tuple, name: str) -> None:
     if tuple(t.shape) != shape or not t.is_contiguous():
         raise _lib.AmbError(f"{name}: expected a contiguous {shape} tensor, got {tuple(t.shape)}")

@@ -5,6 +5,11 @@
 for the input frame (when given) and one per camera, each cell `image_size` square.  A camera cell is the mesh's interpolated
 vertex normals seen from that camera, rasterized at 2x2 samples per pixel, composited on white with the 2x2 coverage as alpha,
 exactly as the reference's Renderer + soft_normal_shading + make_normal_image produce it.  DESIGN.md §16 states every formula.
+
+`render(..., modalities=("normal", "texture"), visual=...)` also writes `grid_texture.mp4`: the same rasterization shaded with
+the glTF base colour (its texture, mip-mapped and filtered as the sampler says, or its factor) under a two-sided headlight,
+each pixel the mean of its four samples (DESIGN.md §16, "Texture shading").  Each mesh is rasterized once per frame for
+every modality.
 Differences from the reference:
   - the video is encoded by OpenCV's `mp4v` writer (the reference uses imageio, which this project does not depend on): same
     file name, frame rate, frame size and frame count, different codec;
@@ -14,8 +19,10 @@ Differences from the reference:
 """
 from __future__ import annotations
 
+import io
 import logging
 import math
+from dataclasses import dataclass
 from pathlib import Path
 from typing import Optional
 
@@ -28,6 +35,8 @@ logger = logging.getLogger(__name__)
 
 ELEVATION_CYCLE = (70, 55, 85, 40)
 FPS = 12
+MODALITIES = ("normal", "texture")
+MAX_TEXTURE_SIDE = 16384
 
 
 def uniform_cameras(distance: float = 3.0, n_cameras: int = 16,
@@ -98,6 +107,69 @@ def write_video(frames: np.ndarray, path: Path, fps: int = FPS) -> None:
         writer.release()
 
 
+@dataclass
+class TextureShading:
+    """What the texture modality samples: the decoded base-colour image ((h, w, 3) uint8, or None for a flat colour), the
+    sampler's glTF enums and the base colour factor (RGB)."""
+    image: Optional[np.ndarray]
+    mag_filter: int
+    min_filter: int
+    wrap_s: int
+    wrap_t: int
+    base_color: tuple
+
+
+def texture_shading(visual) -> TextureShading:
+    """The base colour of a `gltf.GltfVisual` (or None) as the texture modality uses it.
+
+    No visual or no material: the animated GLB's default material colour.  A material: its `baseColorFactor` RGB, times
+    its `baseColorTexture` when that is usable (no `texCoord` other than 0, no textureInfo `extensions`, an image source
+    and UVs); an unusable texture is ignored with one warning.  The image is decoded by Pillow to RGB (alpha ignored).
+    Raises ValueError on an image side above 16384 or a sampler enum glTF does not define."""
+    from .gltf import DEFAULT_MATERIAL, GltfVisual
+
+    default = (ops.LINEAR, ops.LINEAR_MIPMAP_NEAREST, ops.REPEAT, ops.REPEAT)
+    if visual is not None and not isinstance(visual, GltfVisual):
+        raise ValueError(f"render: visual must be a gltf.GltfVisual, got {type(visual).__name__}")
+    if visual is None or visual.material is None:
+        return TextureShading(None, *default, tuple(DEFAULT_MATERIAL["pbrMetallicRoughness"]["baseColorFactor"][:3]))
+    pbr = visual.material.get("pbrMetallicRoughness", {})
+    base = tuple(float(x) for x in pbr.get("baseColorFactor", [1.0, 1.0, 1.0, 1.0])[:3])
+    info = pbr.get("baseColorTexture")
+    if info is None:
+        return TextureShading(None, *default, base)
+    tex = visual.textures[info["index"]] if 0 <= info.get("index", -1) < len(visual.textures) else {}
+    why = ("it uses texCoord %s" % info["texCoord"] if info.get("texCoord", 0) != 0 else
+           "its textureInfo has extensions (%s)" % ", ".join(info["extensions"]) if info.get("extensions") else
+           "it has no image source" if "source" not in tex else
+           "the mesh has no UVs" if visual.uv is None else None)
+    if why is not None:
+        logger.warning(f"render: the base colour texture is ignored because {why}; shading with the base colour factor")
+        return TextureShading(None, *default, base)
+    smp = visual.samplers[tex["sampler"]] if "sampler" in tex else {}
+    mode = (smp.get("magFilter", default[0]), smp.get("minFilter", default[1]), smp.get("wrapS", default[2]),
+            smp.get("wrapT", default[3]))
+    for value, allowed, name in zip(mode, (ops.MAG_FILTERS, ops.MIN_FILTERS, ops.WRAP_MODES, ops.WRAP_MODES),
+                                    ("magFilter", "minFilter", "wrapS", "wrapT")):
+        if value not in allowed:
+            raise ValueError(f"render: sampler {name} {value} is not a glTF value ({', '.join(map(str, allowed))})")
+    from PIL import Image
+
+    with Image.open(io.BytesIO(visual.image_bytes[tex["source"]])) as img:
+        if max(img.size) > MAX_TEXTURE_SIDE:
+            raise ValueError(f"render: texture of {img.size[0]} x {img.size[1]} texels; each side must be <= {MAX_TEXTURE_SIDE}")
+        rgb = np.array(img.convert("RGB"))
+    return TextureShading(rgb, *mode, base)
+
+
+def _modalities(modalities) -> tuple:
+    mods = tuple(modalities) if not isinstance(modalities, str) else (modalities,)
+    unknown = [m for m in mods if m not in MODALITIES]
+    if unknown or not mods or len(set(mods)) != len(mods):
+        raise ValueError(f"render: modalities must be distinct names from {MODALITIES}, got {modalities!r}")
+    return mods
+
+
 class B200MeshVisualizer:
     """Drop-in for the reference's `ActionMeshVisualizer` (same constructor and `render(meshes, device, output_dir,
     input_frames)`), rendering on `device`."""
@@ -116,44 +188,74 @@ class B200MeshVisualizer:
         return torch.from_numpy(table).to(self.device), focal.pop()
 
     @torch.no_grad()
-    def render_frames(self, meshes: list, input_frames: Optional[list] = None) -> torch.Tensor:
-        """The video's frames before encoding -> host uint8 (n_frames, S, n_cols * S, 3), n_cols = cameras (+ 1 for the input
-        frame column when `input_frames` is given)."""
+    def render_frames(self, meshes: list, input_frames: Optional[list] = None, *, modalities=("normal",), visual=None):
+        """The video's frames before encoding, per modality: host uint8 (n_frames, S, n_cols * S, 3), n_cols = cameras (+ 1
+        for the input frame column when `input_frames` is given).  One modality -> its grid; several -> a tuple of grids in
+        the order given.  `visual` (a `gltf.GltfVisual`, its uv one row per mesh vertex) gives "texture" its base colour."""
+        mods = _modalities(modalities)
+        S, n = self.image_size, len(meshes)
+        arrays = [mesh_arrays(m) for m in meshes]
+        uv = None if visual is None or getattr(visual, "uv", None) is None else np.asarray(visual.uv, dtype=np.float32)
+        if uv is not None:
+            if not np.isfinite(uv).all():
+                raise ValueError("render: visual.uv has non-finite values")
+            for verts, _ in arrays:
+                if uv.shape != (len(verts), 2):
+                    raise ValueError(f"render: visual.uv has shape {uv.shape}, but a mesh has {len(verts)} vertices")
         if self.device.type != "cuda":
             raise ops._lib.AmbError("B200MeshVisualizer renders on CUDA (sm_90a) only; there is no CPU fallback")
         if not self.cameras:
             raise ValueError("render: no camera selected")
-        S, n = self.image_size, len(meshes)
-        arrays = [mesh_arrays(m) for m in meshes]
+        shading = texture_shading(visual) if "texture" in mods else None
         frames = resample_list(list(input_frames), n) if input_frames is not None else None
         col0 = 1 if frames is not None else 0
         n_cols = col0 + len(self.cameras)
         with torch.cuda.device(self.device):
             cams, focal = self._camera_table()
-            grid = torch.empty(n, S, n_cols * S, 3, dtype=torch.uint8, device=self.device)
+            grids = [torch.empty(n, S, n_cols * S, 3, dtype=torch.uint8, device=self.device) for _ in mods]
+            tex = {}
+            if shading is not None:
+                tex = dict(mag_filter=shading.mag_filter, min_filter=shading.min_filter, wrap_s=shading.wrap_s,
+                           wrap_t=shading.wrap_t, base_color=shading.base_color)
+                if shading.image is not None:  # the mip chain is built once per call
+                    levels, table = ops.texture_levels(torch.from_numpy(shading.image).to(self.device))
+                    tex.update(uv=torch.from_numpy(uv).to(self.device), levels=levels, table=table)
             for k, (verts, faces) in enumerate(arrays):
                 v, f = torch.from_numpy(verts).to(self.device), torch.from_numpy(faces).to(self.device)  # no faces: white cells
                 normals = ops.vertex_normals(v, f)
                 pix_to_face = ops.rasterize(v, f, cams, focal, S)
-                ops.shade_normals(v, f, normals, cams, focal, pix_to_face, out=grid[k], column=col0)
-            grid = grid.cpu()
+                for grid, mod in zip(grids, mods):
+                    if mod == "normal":
+                        ops.shade_normals(v, f, normals, cams, focal, pix_to_face, out=grid[k], column=col0)
+                    else:
+                        ops.shade_texture(v, f, normals, cams, focal, pix_to_face, out=grid[k], column=col0, **tex)
+            grids = [g.cpu() for g in grids]
         if frames is not None:
             for k, frame in enumerate(frames):
-                grid[k, :, :S] = torch.from_numpy(_frame_rgb(frame, S))
-        return grid
+                cell = torch.from_numpy(_frame_rgb(frame, S))
+                for grid in grids:
+                    grid[k, :, :S] = cell
+        return grids[0] if len(grids) == 1 else tuple(grids)
 
     @torch.no_grad()
-    def render(self, meshes: list, device=None, output_dir: str = ".", input_frames: Optional[list] = None) -> list[Path]:
-        """Render the meshes and write output_dir/grid_normal.mp4 (12 fps) -> [its path] ([] when there are no meshes).
-        `device`, when given, replaces the constructor's."""
+    def render(self, meshes: list, device=None, output_dir: str = ".", input_frames: Optional[list] = None, *,
+               modalities=("normal",), visual=None) -> list[Path]:
+        """Render the meshes and write output_dir/grid_{modality}.mp4 (12 fps) for each modality, in the order given ->
+        their paths ([] when there are no meshes).  `device`, when given, replaces the constructor's; `visual` as for
+        `render_frames`."""
+        mods = _modalities(modalities)
         if device is not None:
             self.device = torch.device(device)
         if not len(meshes):
             return []
-        grid = self.render_frames(meshes, input_frames)
+        grids = self.render_frames(meshes, input_frames, modalities=mods, visual=visual)
+        grids = (grids,) if len(mods) == 1 else grids
         out_dir = Path(output_dir)
         out_dir.mkdir(parents=True, exist_ok=True)
-        path = out_dir / "grid_normal.mp4"
-        write_video(grid.numpy(), path)
-        logger.info(f"Saved render: {path}")
-        return [path]
+        paths = []
+        for mod, grid in zip(mods, grids):
+            path = out_dir / f"grid_{mod}.mp4"
+            write_video(grid.numpy(), path)
+            logger.info(f"Saved render: {path}")
+            paths.append(path)
+        return paths

@@ -369,6 +369,29 @@ int amb_render_shade_normals(const float* vertices, int64_t n_vertices, const in
                              const int32_t* pix_to_face, uint8_t* out, int64_t row_stride, int64_t view_stride,
                              amb_stream_t stream);
 
+/* ---- texture shading of the same rasterization (csrc/render.cu; DESIGN.md §16, "Texture shading") ---------------------------
+ * A texture is a mip chain of row-major RGB uint8 levels in one DEVICE buffer, described by a HOST level table of n_levels
+ * rows of three int64: (byte offset, width, height).  The table must describe the full chain: level 0 of 1..16384 texels a
+ * side, level l + 1 of (max(1, w >> 1), max(1, h >> 1)), down to 1 x 1 (so n_levels <= 15), at ascending byte offsets whose
+ * ranges do not overlap.
+ *  render_texture_levels: fills levels 1 .. n_levels - 1 from level 0, which the caller has written: each texel is
+ *    floor((a + b + c + d + 2) / 4) per channel over the previous level's texels (min(2x + dx, w - 1), min(2y + dy, h - 1)).
+ *    One launch per level after the first.
+ *  render_shade_texture: for each view c and output pixel (i, j) of S x S, the uint8 RGB mean of the shaded colours of its
+ *    four samples, written with render_shade_normals' layout and strides.  Vertices, faces, normals, cameras, focal, S and
+ *    pix_to_face as for render_shade_normals; uv: (V, 2) fp32 DEVICE array (glTF TEXCOORD_0, (0, 0) at the first texel).
+ *    mag_filter is 9728 (NEAREST) or 9729 (LINEAR); min_filter one of 9728, 9729 and 9984..9987 (*_MIPMAP_LINEAR behaves as
+ *    *_MIPMAP_NEAREST); wrap_s / wrap_t are 10497 (REPEAT), 33071 (CLAMP_TO_EDGE) or 33648 (MIRRORED_REPEAT).  base_r/g/b
+ *    is the material's base colour factor.  n_levels = 0 shades without a texture (colour = base factor times the
+ *    headlight); levels, level_table and uv may then be NULL.  With zero faces every cell is white. */
+int amb_render_texture_levels(uint8_t* levels, const int64_t* level_table, int n_levels, amb_stream_t stream);
+int amb_render_shade_texture(const float* vertices, int64_t n_vertices, const int32_t* faces, int64_t n_faces,
+                             const float* normals, const float* uv, const float* cameras, int n_cameras, float focal,
+                             int image_size, const int32_t* pix_to_face, const uint8_t* levels, const int64_t* level_table,
+                             int n_levels, int mag_filter, int min_filter, int wrap_s, int wrap_t, float base_r,
+                             float base_g, float base_b, uint8_t* out, int64_t row_stride, int64_t view_stride,
+                             amb_stream_t stream);
+
 /* ---- background removal: RMBG-1.4 around split-bf16 GEMM convolutions, mask head and refinement (csrc/rmbg.cu) -------------
  * Replaces BackgroundRemover.forward (actionmesh/preprocessing/background_removal.py:84-112) with BriaRMBG
  * (third_party/TripoSG/scripts/briarmbg.py:355-463).  Every 3x3 convolution is rmbg_im2col_split followed by amb_gemm_bf16 on

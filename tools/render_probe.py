@@ -1,10 +1,12 @@
 """Time B200MeshVisualizer.render_frames (mesh upload, vertex normals, rasterization of 3 views at 2S x 2S samples, shading,
 grid download) with CUDA events, on a depth-9 Stage 0 mesh (~1.75 M faces, the rippled ball the geometry tests refine) and
-on that mesh decimated to 40 000 faces, at 16 and 31 frames x 3 cameras x S = 256.  Prints the card and its power limit
-with the numbers.
+on that mesh decimated to 40 000 faces, at 16 and 31 frames x 3 cameras x S = 256.  Then the texture modality on the
+decimated mesh: normal only against normal + texture (a --texture-size square JPEG, decoded and mip-mapped in every call,
+on spherical UVs), the two alternated.  Prints the card and its power limit with the numbers.
 
-    python tools/render_probe.py [--repeats 3]
+    python tools/render_probe.py [--repeats 3] [--texture-size 2048]
 """
+import io
 import argparse
 import os
 import subprocess
@@ -35,6 +37,7 @@ def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--image-size", type=int, default=256)
+    ap.add_argument("--texture-size", type=int, default=2048)
     args = ap.parse_args()
 
     import geometry_exact as gx
@@ -70,6 +73,50 @@ def main() -> None:
             ms = float(np.median(times))
             print(f"{name}: {len(f):,} faces, {n} frames x 3 views, S = {args.image_size}: {ms:.1f} ms per clip "
                   f"(min {min(times):.1f}), {ms / (3 * n):.2f} ms per view")
+
+    v, f = meshes["decimated"]
+    visual = _textured(v, args.texture_size)
+    for n in (16, 31):
+        clip = _frames(v, f, n)
+        runs = {("normal",): [], ("normal", "texture"): []}
+        for mods in runs:
+            vis.render_frames(clip[:2], modalities=mods, visual=visual)  # warm-up
+        for _ in range(args.repeats):
+            for mods, times in runs.items():
+                times.append(_timed(lambda: vis.render_frames(clip, modalities=mods, visual=visual)))
+        for mods, times in runs.items():
+            ms = float(np.median(times))
+            print(f"decimated: {len(f):,} faces, {n} frames x 3 views, S = {args.image_size}, {' + '.join(mods)}"
+                  f"{f', {args.texture_size}^2 texture' if 'texture' in mods else ''}: {ms:.1f} ms per clip "
+                  f"(min {min(times):.1f}, max {max(times):.1f})")
+
+
+def _timed(fn) -> float:
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    e0.record()
+    fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1)
+
+
+def _textured(v: np.ndarray, size: int):
+    """A GltfVisual on spherical UVs with a size x size JPEG: a colour gradient with seeded noise."""
+    from PIL import Image
+
+    from actionmesh_b200.gltf import GltfVisual
+
+    c = v - v.mean(0)
+    uv = np.stack([np.arctan2(c[:, 2], c[:, 0]) / (2 * np.pi) + 0.5,
+                   np.arccos(np.clip(c[:, 1] / np.linalg.norm(c, axis=1), -1, 1)) / np.pi], 1).astype(np.float32)
+    y, x = np.mgrid[0:size, 0:size]
+    noise = np.random.default_rng(0).integers(0, 48, (size, size, 3))
+    img = np.stack([x * 200 // size, y * 200 // size, (x + y) * 100 // size], -1) + noise
+    buf = io.BytesIO()
+    Image.fromarray(img.astype(np.uint8)).save(buf, format="JPEG", quality=90)
+    return GltfVisual(uv=uv, material={"pbrMetallicRoughness": {"baseColorTexture": {"index": 0}}},
+                      textures=[{"source": 0}], images=[{"mimeType": "image/jpeg"}], image_bytes=[buf.getvalue()])
 
 
 if __name__ == "__main__":
