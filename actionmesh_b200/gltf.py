@@ -4,6 +4,7 @@
   load_glb(path) -> Mesh                     every triangle primitive of the default scene, node transforms applied
   write_glb(path, mesh)                      one node, one mesh, one triangle primitive (what trimesh exports)
   write_animated_glb(path, vertices, faces)  one morph target per frame and a weights animation (what Blender exports)
+  write_skinned_glb(path, fit, faces)        a rest mesh, its bones and skin weights, and a joint animation
   save_meshes(meshes, output_dir)            mesh_00.glb, mesh_01.glb, ...
   save_deformation(meshes, path)             {stem}_vertices.npy / {stem}_faces.npy
 
@@ -472,6 +473,84 @@ def write_animated_glb(path, vertices, faces, fps: float = 8, visual: Optional[G
                            "channels": [{"sampler": 0, "target": {"node": 0, "path": "weights"}}],
                            "samplers": [{"input": times, "output": b.accessor(weights.reshape(-1, 1), F32, "SCALAR"),
                                          "interpolation": "LINEAR"}]}]
+    b.write(path, gltf)
+
+
+def _quaternions(rot: np.ndarray) -> np.ndarray:
+    """(..., 3, 3) proper rotations -> (..., 4) unit quaternions (x, y, z, w), glTF's order, from the largest of the four
+    squared components (Shepperd's method)."""
+    r = np.asarray(rot, dtype=np.float64)
+    tr = r[..., 0, 0] + r[..., 1, 1] + r[..., 2, 2]
+    sq = np.stack([1 + 2 * r[..., 0, 0] - tr, 1 + 2 * r[..., 1, 1] - tr, 1 + 2 * r[..., 2, 2] - tr, 1 + tr], -1)
+    k = np.argmax(sq, -1)
+    q = np.empty(r.shape[:-2] + (4,))
+    s = np.sqrt(np.maximum(np.take_along_axis(sq, k[..., None], -1)[..., 0], 1e-300))    # 4 |q_k|
+    off = {(0, 1): r[..., 0, 1] + r[..., 1, 0], (0, 2): r[..., 0, 2] + r[..., 2, 0], (1, 2): r[..., 1, 2] + r[..., 2, 1],
+           (0, 3): r[..., 2, 1] - r[..., 1, 2], (1, 3): r[..., 0, 2] - r[..., 2, 0], (2, 3): r[..., 1, 0] - r[..., 0, 1]}
+    for a in range(4):
+        sel = k == a
+        for b in range(4):
+            q[..., b] = np.where(sel, s / 2 if a == b else off[min(a, b), max(a, b)] / (2 * s), q[..., b])
+    return q / np.linalg.norm(q, axis=-1, keepdims=True)
+
+
+def write_skinned_glb(path, fit, faces, fps: float = 8, visual: Optional[GltfVisual] = None) -> None:
+    """Write a `skinning.SkinningFit` on (F, 3) `faces` as a skinned GLB: one rest mesh, n_bones joints and one LINEAR
+    animation, in the coordinates of `write_animated_glb` (DESIGN §20).
+
+    The mesh node carries skin 0; its primitive has POSITION = M p (float32 with min/max), JOINTS_0 (u8) and WEIGHTS_0
+    (float32, each row divided by its sum).  Joint j is a child of the root node "Armature", placed at M c_j (c_j: the bone's
+    rest centre), with inverse bind matrix translate(-M c_j).  Keyframe k at k / fps sets joint j's rotation to the
+    quaternion of M R_j^k M^T (each key's sign chosen closest to the previous key's) and its translation to
+    M (R_j^k c_j + t_j^k), so that the joint matrix is M [R_j^k | t_j^k] M^T.  Without `visual` the material is the animated
+    GLB's default blue, double-sided; with one its UVs, material and textures are kept."""
+    rest = np.asarray(fit.rest, dtype=np.float64)
+    f = np.asarray(faces).reshape(-1, 3)
+    rot, trans, centres = (np.asarray(a, dtype=np.float64) for a in (fit.rotations, fit.translations, fit.centres))
+    T, B = rot.shape[:2]
+    if not len(f):
+        raise ValueError("a skinned GLB needs at least one face")
+    _check_faces(f, len(rest))
+    if B > 256 or fit.joints.shape != (len(rest), 4) or np.asarray(fit.joints).min() < 0 or np.asarray(fit.joints).max() >= B:
+        raise ValueError(f"joints must be (V, 4) indices of the {B} bones (at most 256)")
+    w = np.asarray(fit.weights, dtype=np.float64)
+    total = w.sum(1, keepdims=True)
+    if w.shape != (len(rest), 4) or (w < 0).any() or not (total > 0).all():
+        raise ValueError("weights must be (V, 4), non-negative, with a positive sum per vertex")
+    M = ANIMATED_GLB_MAP
+    b = _GlbBuilder()
+    attributes = {"POSITION": b.accessor((rest @ M.T).astype(np.float32), F32, "VEC3", ARRAY_BUFFER, min_max=True),
+                  "JOINTS_0": b.accessor(np.asarray(fit.joints, dtype=np.uint8), U8, "VEC4", ARRAY_BUFFER),
+                  "WEIGHTS_0": b.accessor((w / total).astype(np.float32), F32, "VEC4", ARRAY_BUFFER)}
+    indices = b.accessor(f.reshape(-1, 1), U32, "SCALAR", ELEMENT_ARRAY_BUFFER)
+    mc = centres @ M.T
+    joint_nodes = list(range(2, 2 + B))
+    gltf: dict = {"scene": 0, "scenes": [{"nodes": [0, 1]}],
+                  "nodes": [{"mesh": 0, "skin": 0, "name": "SkinnedMesh"}, {"name": "Armature", "children": joint_nodes}]
+                  + [{"name": f"Bone_{j}", "translation": mc[j].tolist()} for j in range(B)]}
+    b.add_visual(gltf, attributes, visual, len(rest))
+    if "materials" not in gltf:
+        gltf["materials"] = [copy.deepcopy(DEFAULT_MATERIAL)]
+    gltf["meshes"] = [{"name": "SkinnedMesh", "primitives": [{"attributes": attributes, "indices": indices, "material": 0,
+                                                              "mode": TRIANGLES}]}]
+    ibm = np.tile(np.eye(4), (B, 1, 1))
+    ibm[:, :3, 3] = -mc
+    gltf["skins"] = [{"joints": joint_nodes, "skeleton": 1,
+                      "inverseBindMatrices": b.accessor(ibm.transpose(0, 2, 1).reshape(B, 16).astype(np.float32), F32,
+                                                        "MAT4")}]
+    quat = _quaternions(M @ rot @ M.T)                                                   # (T, B, 4)
+    for k in range(1, T):
+        quat[k] *= np.where((quat[k] * quat[k - 1]).sum(-1) < 0, -1.0, 1.0)[:, None]
+    node_t = (np.einsum("tbij,bj->tbi", rot, centres) + trans) @ M.T                    # (T, B, 3)
+    times = b.accessor((np.arange(T, dtype=np.float64) / fps).astype(np.float32).reshape(-1, 1), F32, "SCALAR",
+                       min_max=True)
+    samplers, channels = [], []
+    for j in range(B):
+        for path_, data, type_ in (("translation", node_t[:, j], "VEC3"), ("rotation", quat[:, j], "VEC4")):
+            samplers.append({"input": times, "output": b.accessor(data.astype(np.float32), F32, type_),
+                             "interpolation": "LINEAR"})
+            channels.append({"sampler": len(samplers) - 1, "target": {"node": joint_nodes[j], "path": path_}})
+    gltf["animations"] = [{"name": "Animation", "channels": channels, "samplers": samplers}]
     b.write(path, gltf)
 
 

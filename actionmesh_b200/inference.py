@@ -1,13 +1,14 @@
 """The command line: video (+ optional .glb mesh) -> animated meshes on disk, on this package alone.
 
     python -m actionmesh_b200.inference --input clip.mp4 [--mesh_input mesh.glb] [--output_dir DIR] [--fast] [--low_ram]
-                                        [--render_texture]
+                                        [--render_texture] [--skinning_bones N]
 
 One entry point for the reference's `inference/video_to_animated_mesh.py` and `inference/video_and_3d_to_animated_mesh.py`
 (`--mesh_input` selects the second), with their flags and defaults plus `--weights_root`.  It writes, in `--output_dir`
 (default outputs/<input stem>): mesh_00.glb ..., deformations_vertices.npy, deformations_faces.npy, animated_mesh.glb and
 grid_normal.mp4, and with `--render_texture` also grid_texture.mp4 (the meshes shaded with the input mesh's texture, or
-with the default colour).  `--blender_path` and `--dtype` are accepted so that the reference's documented command lines run
+with the default colour), and with `--skinning_bones N` also skinned_mesh.glb (the same animation as N bones and skin
+weights fitted on the GPU, `skinning.fit_skinning`).  `--blender_path` and `--dtype` are accepted so that the reference's documented command lines run
 unchanged, and have no effect: the animated GLB is written without Blender, and the CUDA path owns its precision.
 """
 from __future__ import annotations
@@ -23,7 +24,8 @@ import numpy as np
 import torch
 
 from . import render
-from .gltf import load_glb, save_deformation, save_meshes, write_animated_glb
+from . import skinning
+from .gltf import load_glb, save_deformation, save_meshes, write_animated_glb, write_skinned_glb
 from .pipeline import ActionMeshB200Pipeline, ActionMeshB200PipelineWithMeshInput
 from .video_input import load_frames
 
@@ -35,10 +37,11 @@ ANIMATION_FPS = 8
 
 @torch.no_grad()
 def run_actionmesh(pipeline, input: str, output_dir: str, seed: int = 44, mesh_input: Optional[str] = None,
-                   render_texture: bool = False, **overrides) -> list:
+                   render_texture: bool = False, skinning_bones: int = 0, **overrides) -> list:
     """The reference scripts' `run_actionmesh`: load the frames (and the mesh), run `pipeline`, write every output file
     into `output_dir` -> the meshes.  `render_texture` adds grid_texture.mp4, shaded with the input mesh's visual (the one
-    the animated GLB gets).  `overrides` are the pipeline's per-call arguments (stage_0_steps, face_decimation,
+    the animated GLB gets).  `skinning_bones` > 0 adds skinned_mesh.glb: that many bones fitted to the animated GLB's
+    vertices, written with its faces and visual.  `overrides` are the pipeline's per-call arguments (stage_0_steps, face_decimation,
     floaters_threshold, stage_1_steps, guidance_scales, anchor_idx)."""
     frames = load_frames(input, max_frames=MAX_FRAMES)
     visual = None
@@ -55,9 +58,15 @@ def run_actionmesh(pipeline, input: str, output_dir: str, seed: int = 44, mesh_i
     save_meshes(meshes, output_dir)
     save_deformation(meshes, os.path.join(output_dir, "deformations"))
     animated = os.path.join(output_dir, "animated_mesh.glb")
-    write_animated_glb(animated, np.stack([np.asarray(m.vertices) for m in meshes]), faces, fps=ANIMATION_FPS,
-                       visual=visual)
+    vertices = np.stack([np.asarray(m.vertices) for m in meshes])
+    write_animated_glb(animated, vertices, faces, fps=ANIMATION_FPS, visual=visual)
     logger.info(f"Animated GLB saved to {animated}")
+    if skinning_bones > 0:
+        fit = skinning.fit_skinning(vertices, skinning_bones, device=pipeline.device)
+        skinned = os.path.join(output_dir, "skinned_mesh.glb")
+        write_skinned_glb(skinned, fit, faces, fps=ANIMATION_FPS, visual=visual)
+        logger.info(f"Skinned GLB saved to {skinned} ({skinning_bones} bones; RMS error {fit.rms_error:.3e}, max error "
+                    f"{fit.max_error:.3e} of the rest bounding-box diagonal)")
     visualizer = render.B200MeshVisualizer(image_size=256)
     if render_texture:
         visualizer.render(meshes, pipeline.device, output_dir, frames.frames, modalities=("normal", "texture"),
@@ -89,6 +98,8 @@ def parse_args(argv=None) -> argparse.Namespace:
     p.add_argument("--anchor_idx", type=int, default=None, help="Index of the anchor frame. Default: 0")
     p.add_argument("--render_texture", action="store_true",
                    help="Also write grid_texture.mp4: the meshes shaded with the input mesh's texture (or a flat colour).")
+    p.add_argument("--skinning_bones", type=int, default=0,
+                   help="Also write skinned_mesh.glb with this many bones fitted to the animation (at most 256). Default: 0 (off)")
     return p.parse_args(argv)
 
 
@@ -106,7 +117,7 @@ def main(argv=None) -> list:
     overrides = {k: getattr(args, k) for k in ("stage_0_steps", "face_decimation", "floaters_threshold",
                                                "stage_1_steps", "guidance_scales", "anchor_idx")}
     return run_actionmesh(pipeline, args.input, output_dir, seed=args.seed, mesh_input=args.mesh_input,
-                          render_texture=args.render_texture, **overrides)
+                          render_texture=args.render_texture, skinning_bones=args.skinning_bones, **overrides)
 
 
 if __name__ == "__main__":

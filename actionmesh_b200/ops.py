@@ -900,6 +900,111 @@ def icp_transform_points(points: torch.Tensor, transform: torch.Tensor) -> torch
     return out
 
 
+# ---- skinning decomposition (csrc/skinning.cu; DESIGN.md §20) ------------------------------------------------------------------
+# rest (V, 3), vertices (T, V, 3), transforms (T, B, 12) = R row-major then t, weights (V, 4): contiguous fp64; joints (V, 4)
+# int32.  A slot is used when its weight is > 0.
+
+def _skin_sizes(rest: torch.Tensor, vertices: Optional[torch.Tensor], transforms: Optional[torch.Tensor]) -> tuple:
+    V = rest.shape[0] if rest.dim() == 2 else 0
+    _icp_tensor(rest, (V, 3), "rest")
+    T = vertices.shape[0] if vertices is not None and vertices.dim() == 3 else 1
+    if vertices is not None:
+        _icp_tensor(vertices, (T, V, 3), "vertices")
+    B = transforms.shape[1] if transforms is not None and transforms.dim() == 3 else 0
+    if transforms is not None:
+        _icp_tensor(transforms, (T, B, 12), "transforms")
+    return T, V, B
+
+
+def _skin_slots(joints: torch.Tensor, weights: torch.Tensor, V: int) -> None:
+    _icp_tensor(joints, (V, 4), "joints")
+    _icp_tensor(weights, (V, 4), "weights")
+
+
+def skin_scratch(frames: int, n_vertices: int, device) -> torch.Tensor:
+    """The fp64 scratch `skin_bone_update` and `skin_error` need for these sizes."""
+    n = C.c_int64()
+    _lib.check(_abi.amb_skin_scratch_doubles(int(frames), int(n_vertices), C.byref(n)), "amb_skin_scratch_doubles")
+    return torch.empty(n.value, dtype=torch.float64, device=device)
+
+
+def skin_seeds(rest: torch.Tensor, n_bones: int) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Farthest-point sampling of `n_bones` rest vertices from vertex 0 -> (seeds (B) int32, labels (V) int32 = nearest
+    seed, centres (B, 3) fp64 = the seeds' positions)."""
+    dev = _device(rest, "rest")
+    _, V, _ = _skin_sizes(rest, None, None)
+    seeds = torch.empty(n_bones, dtype=torch.int32, device=rest.device)
+    labels = torch.empty(V, dtype=torch.int32, device=rest.device)
+    centres = torch.empty(n_bones, 3, dtype=torch.float64, device=rest.device)
+    dist = torch.empty(V, dtype=torch.float64, device=rest.device)
+    _launch(_abi.amb_skin_seeds, 1, _ptr(rest, torch.float64, "rest", dev), V, int(n_bones),
+            _ptr(dist, torch.float64, "dist", dev), _ptr(seeds, torch.int32, "seeds", dev),
+            _ptr(labels, torch.int32, "labels", dev), _ptr(centres, torch.float64, "centres", dev))
+    return seeds, labels, centres
+
+
+def skin_rigid_error(rest: torch.Tensor, vertices: torch.Tensor, transforms: torch.Tensor):
+    """Per vertex and bone e = sum_t |R p + t - v|^2 -> (argmin (V) int32, min_error (V) fp64, candidates (V, 8) int32: the
+    lowest-error bones in ascending (error, index), -1 past B)."""
+    dev = _device(rest, "rest")
+    T, V, B = _skin_sizes(rest, vertices, transforms)
+    argmin = torch.empty(V, dtype=torch.int32, device=rest.device)
+    min_error = torch.empty(V, dtype=torch.float64, device=rest.device)
+    cand = torch.empty(V, 8, dtype=torch.int32, device=rest.device)
+    _launch(_abi.amb_skin_rigid_error, 1, _ptr(rest, torch.float64, "rest", dev),
+            _ptr(vertices, torch.float64, "vertices", dev), T, V, _ptr(transforms, torch.float64, "transforms", dev), B,
+            _ptr(argmin, torch.int32, "argmin", dev), _ptr(min_error, torch.float64, "min_error", dev),
+            _ptr(cand, torch.int32, "candidates", dev), tag="skin_rigid_error")
+    return argmin, min_error, cand
+
+
+def skin_bone_update(rest: torch.Tensor, vertices: torch.Tensor, transforms: torch.Tensor, joints: torch.Tensor,
+                     weights: torch.Tensor, bone: int, centres: torch.Tensor, scratch: Optional[torch.Tensor] = None) -> None:
+    """Refit bone `bone`'s transform in every frame to the residual the other bones leave (in place on transforms, and
+    centres[bone] = its weighted rest centre); a bone that influences no vertex is left as it is."""
+    dev = _device(rest, "rest")
+    T, V, B = _skin_sizes(rest, vertices, transforms)
+    _skin_slots(joints, weights, V)
+    _icp_tensor(centres, (B, 3), "centres")
+    if scratch is None:
+        scratch = skin_scratch(T, V, rest.device)
+    _launch(_abi.amb_skin_bone_update, 2, _ptr(rest, torch.float64, "rest", dev),
+            _ptr(vertices, torch.float64, "vertices", dev), T, V, _ptr(transforms, torch.float64, "transforms", dev), B,
+            _ptr(joints, torch.int32, "joints", dev), _ptr(weights, torch.float64, "weights", dev), int(bone),
+            _ptr(scratch, torch.float64, "scratch", dev), _ptr(centres, torch.float64, "centres", dev), tag="skin_bone_update")
+
+
+def skin_weight_update(rest: torch.Tensor, vertices: torch.Tensor, transforms: torch.Tensor, candidates: torch.Tensor,
+                       joints: torch.Tensor, weights: torch.Tensor) -> None:
+    """Refit every vertex's <= 4 weights (in place on joints and weights) over its used slots and `candidates` (V, 8)."""
+    dev = _device(rest, "rest")
+    T, V, B = _skin_sizes(rest, vertices, transforms)
+    _skin_slots(joints, weights, V)
+    _icp_tensor(candidates, (V, 8), "candidates")
+    _launch(_abi.amb_skin_weight_update, 1, _ptr(rest, torch.float64, "rest", dev),
+            _ptr(vertices, torch.float64, "vertices", dev), T, V, _ptr(transforms, torch.float64, "transforms", dev), B,
+            _ptr(candidates, torch.int32, "candidates", dev), _ptr(joints, torch.int32, "joints", dev),
+            _ptr(weights, torch.float64, "weights", dev), tag="skin_weight_update")
+
+
+def skin_error(rest: torch.Tensor, vertices: torch.Tensor, transforms: torch.Tensor, joints: torch.Tensor,
+               weights: torch.Tensor, scratch: Optional[torch.Tensor] = None) -> tuple[torch.Tensor, torch.Tensor]:
+    """Reconstruction error of the skinned animation -> (frame_errors (T + 1) fp64 = sum |v^ - v|^2 per frame then their
+    sum, max_error2 (1) fp64 = the largest |v^ - v|^2)."""
+    dev = _device(rest, "rest")
+    T, V, B = _skin_sizes(rest, vertices, transforms)
+    _skin_slots(joints, weights, V)
+    if scratch is None:
+        scratch = skin_scratch(T, V, rest.device)
+    frame_errors = torch.empty(T + 1, dtype=torch.float64, device=rest.device)
+    max_error2 = torch.empty(1, dtype=torch.float64, device=rest.device)
+    _launch(_abi.amb_skin_error, 2, _ptr(rest, torch.float64, "rest", dev), _ptr(vertices, torch.float64, "vertices", dev),
+            T, V, _ptr(transforms, torch.float64, "transforms", dev), B, _ptr(joints, torch.int32, "joints", dev),
+            _ptr(weights, torch.float64, "weights", dev), _ptr(scratch, torch.float64, "scratch", dev),
+            _ptr(frame_errors, torch.float64, "frame_errors", dev), _ptr(max_error2, torch.float64, "max_error2", dev))
+    return frame_errors, max_error2
+
+
 # ---- background removal: RMBG-1.4's resampling, im2col, mask head and refinement (csrc/rmbg.cu) ------------------------------
 # Activations are fp32 NHWC feature maps held as 2-D (H * W, pixel stride) tensors with unit channel stride: a GEMM output
 # padded to 64 columns is read in place, its first C columns being the channels.

@@ -433,6 +433,39 @@ int amb_rmbg_mask_head(const float* feat, int64_t ps, int height, int width, con
 int amb_rmbg_refine_rgba(const uint8_t* rgb, const uint8_t* mask, int height, int width, int refine, int min_size,
                          int32_t* hist, int32_t* labels, int32_t* sizes, uint8_t* rgba, amb_stream_t stream);
 
+/* ---- skinning decomposition: bones and skin weights fitted to a vertex animation (csrc/skinning.cu; DESIGN.md §20) ----------
+ * SSDR (Le & Deng 2012) by alternating least squares; actionmesh_b200/skinning.py drives the calls.  All arithmetic is fp64 with
+ * each operation rounded on its own, in the order DESIGN.md §20 states; no result depends on scheduling.  rest: (V, 3) fp64;
+ * vertices: (T, V, 3) fp64; transforms: (T, B, 12) fp64 = R row-major then t, the bone maps p to R p + t; joints: (V, 4) int32
+ * in [0, B) and weights: (V, 4) fp64, a slot being used when its weight is > 0 (not checked on the device).  1 <= T <= 65535,
+ * 1 <= B <= min(V, 256), V < 2^31 - 256.
+ *  skin_scratch_doubles: the fp64 scratch skin_bone_update and skin_error need for T frames and V vertices.
+ *  skin_seeds: farthest-point sampling of B rest vertices from vertex 0, ties to the lowest index -> seeds (B); labels (V) =
+ *    the nearest seed (ties to the earlier seed); centres (B, 3) = the seeds' positions.  dist: V doubles of scratch.
+ *  skin_rigid_error: e_ij = sum_t |R_j^t p_i + t_j^t - v_i^t|^2 -> argmin (V) = the bone of least e (ties to the lower
+ *    index) and min_error (V) its e; candidates (V, 8) = the min(8, B) bones of least e in ascending (e, index), -1 after.
+ *  skin_bone_update: for bone `bone` and every frame, the rigid transform minimising sum_i |q_i - w_i (R p_i + t)|^2 with
+ *    q_i = v_i - sum of the other used slots' w u, over the vertices whose used slots hold the bone; written to transforms,
+ *    and centres[bone] = sum w^2 p / sum w^2.  A bone with no such vertex keeps its transform and centre.
+ *  skin_weight_update: per vertex, joints and weights (in place) = the lowest-error solution with non-negative weights summing
+ *    to 1 over subsets of <= 4 of its candidates (its used slots, then `candidates` from skin_rigid_error), unused slots 0/0.
+ *  skin_error: frame_errors (T + 1) = sum_i |v^_i - v_i|^2 per frame, then their sum; max_error2 (1) = the largest
+ *    |v^_i - v_i|^2 over vertices and frames, with v^_i = sum of the used slots' w (R p_i + t). */
+int amb_skin_scratch_doubles(int frames, int64_t n_vertices, int64_t* out_doubles);
+int amb_skin_seeds(const double* rest, int64_t n_vertices, int n_bones, double* dist, int32_t* seeds, int32_t* labels,
+                   double* centres, amb_stream_t stream);
+int amb_skin_rigid_error(const double* rest, const double* vertices, int frames, int64_t n_vertices, const double* transforms,
+                         int n_bones, int32_t* argmin, double* min_error, int32_t* candidates, amb_stream_t stream);
+int amb_skin_bone_update(const double* rest, const double* vertices, int frames, int64_t n_vertices, double* transforms,
+                         int n_bones, const int32_t* joints, const double* weights, int bone, double* scratch, double* centres,
+                         amb_stream_t stream);
+int amb_skin_weight_update(const double* rest, const double* vertices, int frames, int64_t n_vertices,
+                           const double* transforms, int n_bones, const int32_t* candidates, int32_t* joints, double* weights,
+                           amb_stream_t stream);
+int amb_skin_error(const double* rest, const double* vertices, int frames, int64_t n_vertices, const double* transforms,
+                   int n_bones, const int32_t* joints, const double* weights, double* scratch, double* frame_errors,
+                   double* max_error2, amb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
