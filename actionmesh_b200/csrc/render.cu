@@ -249,6 +249,7 @@ __global__ void shade_kernel(const float* __restrict__ verts, const int32_t* __r
 constexpr int kMaxTexSide = 16384;
 constexpr int kMaxLevels = 15;  // 16384 -> 1 in 14 halvings
 constexpr float kUvLimit = 32768.0f;
+constexpr int kMaxRecords = 65536;
 
 enum : int {
   kNearest = 9728,
@@ -262,17 +263,11 @@ enum : int {
   kMirroredRepeat = 33648,
 };
 
-// the mip chain as a kernel parameter: level l is h[l] rows of w[l] RGB texels at byte offset off[l] of the level buffer
-struct TexLevels {
-  long long off[kMaxLevels];
-  int w[kMaxLevels], h[kMaxLevels];
-  int n;
-};
-
-struct Sampler {
-  int mag, min, wrap_s, wrap_t;
-  float base[3];
-};
+// a shading record (the header's amb_shade_record): the mip chain, level l being level_height[l] rows of level_width[l] RGB
+// texels at byte offset level_offset[l] of the level buffer (n_levels = 0: no texture), the sampler's enums and the base
+// colour factor.  amb_render_shade_texture passes one by value, amb_render_shade_materials reads one per face.
+using Record = amb_shade_record;
+static_assert(sizeof(((Record*)nullptr)->level_offset) / sizeof(int64_t) == kMaxLevels, "one slot per level");
 
 // level l + 1 texel (x, y) = floor((a + b + c + d + 2) / 4) per channel over level-l texels (min(2x+dx, w-1), min(2y+dy, h-1))
 __global__ void texture_level_kernel(uint8_t* __restrict__ levels, long long src_off, int sw, int sh, long long dst_off,
@@ -302,10 +297,10 @@ __device__ __forceinline__ int wrap_index(int i, int n, int mode) {
 
 // filtered RGB (0..255, not rounded) of level `l` at (u, v): NEAREST texel (floor(u w), floor(v h)), or LINEAR around
 // (u w - 1/2, v h - 1/2) with weights ((t00 (1-fx) + t10 fx) (1-fy)) + ((t01 (1-fx) + t11 fx) fy)
-__device__ __forceinline__ void sample_level(const uint8_t* __restrict__ levels, const TexLevels& tl, int l, bool linear,
+__device__ __forceinline__ void sample_level(const uint8_t* __restrict__ levels, const Record& rec, int l, bool linear,
                                              int wrap_s, int wrap_t, float u, float v, float* rgb) {
-  const int w = tl.w[l], h = tl.h[l];
-  const uint8_t* base = levels + tl.off[l];
+  const int w = rec.level_width[l], h = rec.level_height[l];
+  const uint8_t* base = levels + rec.level_offset[l];
   u = fminf(fmaxf(u, -kUvLimit), kUvLimit);
   v = fminf(fmaxf(v, -kUvLimit), kUvLimit);
   if (!linear) {
@@ -335,8 +330,7 @@ __device__ __forceinline__ void sample_level(const uint8_t* __restrict__ levels,
 __device__ __forceinline__ void texture_sample(const float* __restrict__ verts, const int32_t* __restrict__ faces,
                                                const float* __restrict__ normals, const float* __restrict__ uv,
                                                const float* cp, float focal, int S, int f, int r, int c,
-                                               const uint8_t* __restrict__ levels, const TexLevels& tl,
-                                               const Sampler& sm, float* col) {
+                                               const uint8_t* __restrict__ levels, const Record& rec, float* col) {
   const int n2 = 2 * S;
   const Face s = face_setup(verts, faces, f, cp, focal, n2);
   Bary b;
@@ -351,21 +345,21 @@ __device__ __forceinline__ void texture_sample(const float* __restrict__ verts, 
   const float vz = fa(fa(fm(n.x, cp[2]), fm(n.y, cp[5])), fm(n.z, cp[8]));
   const float len = __fsqrt_rn(fa(fa(fm(vx, vx), fm(vy, vy)), fm(vz, vz)));
   const float shade = fa(0.35f, fm(0.65f, fabsf(fd(vz, len > kShadeEps ? len : kShadeEps))));
-  float base[3] = {sm.base[0], sm.base[1], sm.base[2]};
-  if (tl.n) {
+  float base[3] = {rec.base_color[0], rec.base_color[1], rec.base_color[2]};
+  if (rec.n_levels) {
     const float u0 = uv[2LL * i0], w0 = uv[2LL * i0 + 1], u1 = uv[2LL * i1], w1 = uv[2LL * i1 + 1];
     const float u2 = uv[2LL * i2], w2 = uv[2LL * i2 + 1];
     const float u = fa(fa(fm(b.b0, u0), fm(b.b1, u1)), fm(b.b2, u2)), v = fa(fa(fm(b.b0, w0), fm(b.b1, w1)), fm(b.b2, w2));
     // level of detail of (face, view): projected area A_s in samples against the uv area A_t in level-0 texels
     const float a_s = fm(fm(0.5f, fabsf(edge(s.v0.x, s.v0.y, s.v1, s.v2))), (float)(S * S));
     const float a_t = fm(fm(0.5f, fabsf(fs(fm(fs(u0, u1), fs(w2, w1)), fm(fs(w0, w1), fs(u2, u1))))),
-                         (float)((long long)tl.w[0] * tl.h[0]));
-    int level = 0, filter = sm.mag;  // magnified, or a face with a depth <= 0
+                         (float)((long long)rec.level_width[0] * rec.level_height[0]));
+    int level = 0, filter = rec.mag_filter;  // magnified, or a face with a depth <= 0
     if (s.v0.z > 0.0f && s.v1.z > 0.0f && s.v2.z > 0.0f && !(a_t <= a_s)) {
-      filter = sm.min;
-      if (sm.min >= kNearestMipNearest) {
+      filter = rec.min_filter;
+      if (rec.min_filter >= kNearestMipNearest) {
         float lim = a_s;
-        while (level < tl.n - 1 && !(a_t <= lim)) {
+        while (level < rec.n_levels - 1 && !(a_t <= lim)) {
           lim = fm(lim, 4.0f);
           ++level;
         }
@@ -373,7 +367,7 @@ __device__ __forceinline__ void texture_sample(const float* __restrict__ verts, 
     }
     const bool linear = filter == kLinear || filter == kLinearMipNearest || filter == kLinearMipLinear;
     float t[3];
-    sample_level(levels, tl, level, linear, sm.wrap_s, sm.wrap_t, u, v, t);
+    sample_level(levels, rec, level, linear, rec.wrap_s, rec.wrap_t, u, v, t);
 #pragma unroll
     for (int k = 0; k < 3; ++k) base[k] = fm(base[k], fd(t[k], 255.0f));
   }
@@ -381,14 +375,16 @@ __device__ __forceinline__ void texture_sample(const float* __restrict__ verts, 
   for (int k = 0; k < 3; ++k) col[k] = fm(base[k], shade);
 }
 
-// one thread per output pixel (view, i, j): the mean of its four samples' shaded colours (white where no face), truncated
-__global__ void __launch_bounds__(256) shade_texture_kernel(const float* __restrict__ verts, const int32_t* __restrict__ faces,
-                                                            const float* __restrict__ normals, const float* __restrict__ uv,
-                                                            const float* __restrict__ cams, int n_cams, float focal, int S,
-                                                            const int32_t* __restrict__ pix_to_face,
-                                                            const uint8_t* __restrict__ levels, const TexLevels tl,
-                                                            const Sampler sm, uint8_t* __restrict__ out,
-                                                            long long row_stride, int view_stride) {
+// one thread per output pixel (view, i, j): the mean of its four samples' shaded colours (white where no face), truncated.
+// Each covered sample shades with `rec` when face_record is null (amb_render_shade_texture), else with
+// records[face_record[f]] (amb_render_shade_materials).
+__device__ __forceinline__ void shade_texture_pixels(const float* __restrict__ verts, const int32_t* __restrict__ faces,
+                                                     const float* __restrict__ normals, const float* __restrict__ uv,
+                                                     const float* __restrict__ cams, int n_cams, float focal, int S,
+                                                     const int32_t* __restrict__ pix_to_face,
+                                                     const int32_t* __restrict__ face_record, const Record* __restrict__ records,
+                                                     const uint8_t* __restrict__ levels, const Record& rec,
+                                                     uint8_t* __restrict__ out, long long row_stride, int view_stride) {
   const int n2 = 2 * S;
   const long long n = (long long)n_cams * S * S;
   for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < n; p += (long long)gridDim.x * blockDim.x) {
@@ -401,7 +397,9 @@ __global__ void __launch_bounds__(256) shade_texture_kernel(const float* __restr
       const int r = 2 * i + (q >> 1), c = 2 * j + (q & 1);
       const int f = pf[(long long)r * n2 + c];
       float col[3] = {1.0f, 1.0f, 1.0f};
-      if (f >= 0) texture_sample(verts, faces, normals, uv, cp, focal, S, f, r, c, levels, tl, sm, col);
+      if (f >= 0)
+        texture_sample(verts, faces, normals, uv, cp, focal, S, f, r, c, levels, face_record ? records[face_record[f]] : rec,
+                       col);
 #pragma unroll
       for (int k = 0; k < 3; ++k) acc[k] = q ? fa(acc[k], col[k]) : col[k];
     }
@@ -409,6 +407,28 @@ __global__ void __launch_bounds__(256) shade_texture_kernel(const float* __restr
 #pragma unroll
     for (int k = 0; k < 3; ++k) o[k] = (uint8_t)(int)fm(fminf(fmaxf(fm(acc[k], 0.25f), 0.0f), 1.0f), 255.0f);
   }
+}
+
+__global__ void __launch_bounds__(256) shade_texture_kernel(const float* __restrict__ verts, const int32_t* __restrict__ faces,
+                                                            const float* __restrict__ normals, const float* __restrict__ uv,
+                                                            const float* __restrict__ cams, int n_cams, float focal, int S,
+                                                            const int32_t* __restrict__ pix_to_face,
+                                                            const uint8_t* __restrict__ levels, const Record rec,
+                                                            uint8_t* __restrict__ out, long long row_stride, int view_stride) {
+  shade_texture_pixels(verts, faces, normals, uv, cams, n_cams, focal, S, pix_to_face, nullptr, nullptr, levels, rec, out,
+                       row_stride, view_stride);
+}
+
+__global__ void __launch_bounds__(256) shade_materials_kernel(const float* __restrict__ verts, const int32_t* __restrict__ faces,
+                                                              const float* __restrict__ normals, const float* __restrict__ uv,
+                                                              const float* __restrict__ cams, int n_cams, float focal, int S,
+                                                              const int32_t* __restrict__ pix_to_face,
+                                                              const int32_t* __restrict__ face_record,
+                                                              const Record* __restrict__ records,
+                                                              const uint8_t* __restrict__ levels, uint8_t* __restrict__ out,
+                                                              long long row_stride, int view_stride) {
+  shade_texture_pixels(verts, faces, normals, uv, cams, n_cams, focal, S, pix_to_face, face_record, records, levels,
+                       records[0], out, row_stride, view_stride);
 }
 
 constexpr int kThreads = 256;
@@ -419,23 +439,25 @@ bool render_sizes_ok(int64_t n_vertices, int64_t n_faces) {
 
 // a full mip chain: level 0 of 1..16384 texels a side, each next level halved (at least 1), down to 1 x 1, in ascending
 // non-overlapping byte ranges; false with the reason in *why
-bool level_table_ok(const int64_t* table, int n_levels, TexLevels* tl, const char** why) {
+bool level_table_ok(const int64_t* table, int n_levels, Record* rec, const char** why) {
   *why = "";
   if (n_levels < 1 || n_levels > kMaxLevels) return *why = "n_levels outside [1, 15]", false;
   long long end = 0;
   for (int l = 0; l < n_levels; ++l) {
     const int64_t off = table[3 * l], w = table[3 * l + 1], h = table[3 * l + 2];
     if (l == 0 && (w < 1 || h < 1 || w > kMaxTexSide || h > kMaxTexSide)) return *why = "level 0 size outside [1, 16384]", false;
-    if (l > 0 && (w != (tl->w[l - 1] > 1 ? tl->w[l - 1] >> 1 : 1) || h != (tl->h[l - 1] > 1 ? tl->h[l - 1] >> 1 : 1)))
+    if (l > 0 && (w != (rec->level_width[l - 1] > 1 ? rec->level_width[l - 1] >> 1 : 1) ||
+                  h != (rec->level_height[l - 1] > 1 ? rec->level_height[l - 1] >> 1 : 1)))
       return *why = "a level is not the previous one halved", false;
     if (off < end) return *why = "level byte ranges overlap or descend", false;
-    tl->off[l] = off;
-    tl->w[l] = (int)w;
-    tl->h[l] = (int)h;
+    rec->level_offset[l] = off;
+    rec->level_width[l] = (int)w;
+    rec->level_height[l] = (int)h;
     end = off + 3 * w * h;
   }
-  if (tl->w[n_levels - 1] != 1 || tl->h[n_levels - 1] != 1) return *why = "the chain does not end at 1 x 1", false;
-  tl->n = n_levels;
+  if (rec->level_width[n_levels - 1] != 1 || rec->level_height[n_levels - 1] != 1)
+    return *why = "the chain does not end at 1 x 1", false;
+  rec->n_levels = n_levels;
   return true;
 }
 
@@ -512,12 +534,14 @@ int amb_render_shade_normals(const float* vertices, int64_t n_vertices, const in
 
 int amb_render_texture_levels(uint8_t* levels, const int64_t* level_table, int n_levels, amb_stream_t stream) {
   AMB_CHECK_ARG(levels && level_table, "render_texture_levels: null pointer");
-  TexLevels tl;
+  Record tl;
   const char* why;
   AMB_CHECK_ARG(level_table_ok(level_table, n_levels, &tl, &why), "render_texture_levels: bad level table (%s)", why);
   for (int l = 1; l < n_levels; ++l) {
-    texture_level_kernel<<<blocks_for((long long)tl.w[l] * tl.h[l], kThreads), kThreads, 0, (cudaStream_t)stream>>>(
-        levels, tl.off[l - 1], tl.w[l - 1], tl.h[l - 1], tl.off[l], tl.w[l], tl.h[l]);
+    texture_level_kernel<<<blocks_for((long long)tl.level_width[l] * tl.level_height[l], kThreads), kThreads, 0,
+                           (cudaStream_t)stream>>>(levels, tl.level_offset[l - 1], tl.level_width[l - 1],
+                                                   tl.level_height[l - 1], tl.level_offset[l], tl.level_width[l],
+                                                   tl.level_height[l]);
     AMB_CHECK_CUDA(cudaGetLastError());
   }
   return AMB_OK;
@@ -548,17 +572,49 @@ int amb_render_shade_texture(const float* vertices, int64_t n_vertices, const in
   for (int wrap : {wrap_s, wrap_t})
     AMB_CHECK_ARG(wrap == kRepeat || wrap == kClampToEdge || wrap == kMirroredRepeat, "render_shade_texture: bad wrap mode %d",
                   wrap);
-  TexLevels tl;
-  tl.n = 0;
+  Record rec = {};
   if (n_levels) {
     const char* why;
-    AMB_CHECK_ARG(level_table_ok(level_table, n_levels, &tl, &why), "render_shade_texture: bad level table (%s)", why);
+    AMB_CHECK_ARG(level_table_ok(level_table, n_levels, &rec, &why), "render_shade_texture: bad level table (%s)", why);
   }
-  const Sampler sm = {mag_filter, min_filter, wrap_s, wrap_t, {base_r, base_g, base_b}};
+  rec.mag_filter = mag_filter;
+  rec.min_filter = min_filter;
+  rec.wrap_s = wrap_s;
+  rec.wrap_t = wrap_t;
+  rec.base_color[0] = base_r;
+  rec.base_color[1] = base_g;
+  rec.base_color[2] = base_b;
   const long long n = (long long)n_cameras * image_size * image_size;
   shade_texture_kernel<<<blocks_for(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
-      vertices, faces, normals, uv, cameras, n_cameras, focal, image_size, pix_to_face, levels, tl, sm, out, row_stride,
+      vertices, faces, normals, uv, cameras, n_cameras, focal, image_size, pix_to_face, levels, rec, out, row_stride,
       (int)view_stride);
+  AMB_CHECK_CUDA(cudaGetLastError());
+  return AMB_OK;
+}
+
+int amb_render_shade_materials(const float* vertices, int64_t n_vertices, const int32_t* faces, int64_t n_faces,
+                               const float* normals, const float* uv, const float* cameras, int n_cameras, float focal,
+                               int image_size, const int32_t* pix_to_face, const int32_t* face_record,
+                               const void* records, int n_records, const uint8_t* levels, uint8_t* out,
+                               int64_t row_stride, int64_t view_stride, amb_stream_t stream) {
+  AMB_CHECK_ARG((!n_faces || (vertices && faces && normals && face_record)) && records && cameras && pix_to_face && out,
+                "render_shade_materials: null pointer");
+  AMB_CHECK_ARG(render_sizes_ok(n_vertices, n_faces), "render_shade_materials: bad mesh size (%lld vertices, %lld faces)",
+                (long long)n_vertices, (long long)n_faces);
+  AMB_CHECK_ARG(n_cameras >= 1 && image_size >= 1,
+                "render_shade_materials: need n_cameras >= 1 and image_size >= 1 (got %d, %d)", n_cameras, image_size);
+  const long long n2 = 2LL * image_size;
+  AMB_CHECK_ARG((long long)n_cameras * n2 * n2 < (1LL << 31),
+                "render_shade_materials: %d cameras x %lld samples overflow int32", n_cameras, n2 * n2);
+  AMB_CHECK_ARG(row_stride >= 3LL * image_size && view_stride >= 0 && view_stride < (1LL << 31) &&
+                    (n_cameras == 1 || view_stride >= 3LL * image_size),
+                "render_shade_materials: bad strides (row %lld, view %lld)", (long long)row_stride, (long long)view_stride);
+  AMB_CHECK_ARG(n_records >= 1 && n_records <= kMaxRecords, "render_shade_materials: n_records %d outside [1, %d]", n_records,
+                kMaxRecords);
+  const long long n = (long long)n_cameras * image_size * image_size;
+  shade_materials_kernel<<<blocks_for(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
+      vertices, faces, normals, uv, cameras, n_cameras, focal, image_size, pix_to_face, face_record,
+      static_cast<const Record*>(records), levels, out, row_stride, (int)view_stride);
   AMB_CHECK_CUDA(cudaGetLastError());
   return AMB_OK;
 }

@@ -2,7 +2,7 @@
 `actionmesh/io/mesh_io.py` (trimesh) and `actionmesh/io/glb_export.py` (Blender) without either dependency.
 
   load_glb(path) -> Mesh                     every triangle primitive of the default scene, node transforms applied
-  write_glb(path, mesh)                      one node, one mesh, one triangle primitive (what trimesh exports)
+  write_glb(path, mesh)                      one node, one mesh, one triangle primitive per material (what trimesh exports)
   write_animated_glb(path, vertices, faces)  one morph target per frame and a weights animation (what Blender exports)
   write_skinned_glb(path, fit, faces)        a rest mesh, its bones and skin weights, and a joint animation
   save_meshes(meshes, output_dir)            mesh_00.glb, mesh_01.glb, ...
@@ -62,6 +62,54 @@ class GltfVisual:
     samplers: list = field(default_factory=list)
     images: list = field(default_factory=list)
     image_bytes: list = field(default_factory=list)
+
+
+@dataclass
+class GltfMultiVisual:
+    """The texture side of a mesh made of P >= 2 glTF primitives, in `load_glb`'s concatenation order; the writers give each
+    primitive back its own range and material (DESIGN §19).
+
+    vertex_ranges / face_ranges: (P, 2) int64 (start, count), contiguous and tiling the mesh's vertices and faces; the faces
+    of primitive p index only its vertex range.  uv: (V, 2) float32 TEXCOORD_0 over all vertices (0 on the rows of
+    primitives without it), or None when no primitive has one; has_uv: (P,) bool.  primitive_material: P entries, each an
+    index into `materials` or None.  materials / textures / samplers / images: the glTF JSON, re-indexed from 0 as in
+    `GltfVisual`, each entry stored once however many primitives or textures share it; image i's bytes are `image_bytes[i]`."""
+    vertex_ranges: np.ndarray
+    face_ranges: np.ndarray
+    uv: Optional[np.ndarray] = None
+    has_uv: np.ndarray = field(default_factory=lambda: np.zeros(0, bool))
+    primitive_material: list = field(default_factory=list)
+    materials: list = field(default_factory=list)
+    textures: list = field(default_factory=list)
+    samplers: list = field(default_factory=list)
+    images: list = field(default_factory=list)
+    image_bytes: list = field(default_factory=list)
+
+
+def check_multi_visual(visual: GltfMultiVisual, n_vertices: int, faces: np.ndarray) -> None:
+    """ValueError unless `visual`'s ranges tile `n_vertices` vertices and the (F, 3) `faces`, each range non-empty, each
+    primitive's faces inside its own vertex range, and its per-primitive fields have P entries."""
+    vr, fr = np.asarray(visual.vertex_ranges), np.asarray(visual.face_ranges)
+    P = len(vr)
+    if vr.shape != (P, 2) or fr.shape != (P, 2) or P < 1:
+        raise ValueError(f"visual: vertex_ranges {vr.shape} and face_ranges {fr.shape} must both be (P, 2), P >= 1")
+    for name, r, total in (("vertex", vr, n_vertices), ("face", fr, len(faces))):
+        starts = np.concatenate([[0], np.cumsum(r[:, 1])[:-1]])
+        if (r[:, 1] < 1).any() or not np.array_equal(r[:, 0], starts) or int(r[:, 1].sum()) != total:
+            raise ValueError(f"visual: the {name} ranges do not tile the mesh's {total} {name}s")
+    if len(np.asarray(visual.has_uv)) != P or len(visual.primitive_material) != P:
+        raise ValueError(f"visual: has_uv and primitive_material need {P} entries")
+    if any(m is not None and not 0 <= m < len(visual.materials) for m in visual.primitive_material):
+        raise ValueError(f"visual: a primitive's material is outside the {len(visual.materials)} materials")
+    if visual.uv is not None and np.shape(visual.uv) != (n_vertices, 2):
+        raise ValueError(f"visual.uv has shape {np.shape(visual.uv)}, expected ({n_vertices}, 2)")
+    if np.asarray(visual.has_uv).any() and visual.uv is None:
+        raise ValueError("visual: a primitive has UVs but visual.uv is None")
+    if len(faces):
+        owner = np.repeat(np.arange(P), fr[:, 1])
+        lo, hi = vr[owner, 0], vr[owner, 0] + vr[owner, 1]
+        if (faces.min(1) < lo).any() or (faces.max(1) >= hi).any():
+            raise ValueError("visual: a face indexes a vertex outside its primitive's range")
 
 
 # ------------------------------------------------------------------------------------------------------------------ reading
@@ -222,9 +270,62 @@ def _mesh_instances(gltf: dict, path) -> list:
     return out
 
 
+class _Collector:
+    """Copies materials and what they reference out of one file into `out` (its textures / samplers / images /
+    image_bytes lists), re-indexed from 0 in first-use order, each source entry once."""
+
+    def __init__(self, reader: _Reader, out):
+        self.reader, self.out = reader, out
+        self.tex_map, self.smp_map, self.img_map = {}, {}, {}
+
+    def image(self, i):
+        if i not in self.img_map:
+            img = self.reader.gltf["images"][i]
+            data = (self.reader.view_bytes(img["bufferView"]) if "bufferView" in img
+                    else _read_uri(img["uri"], self.reader.path))
+            entry = {"mimeType": img.get("mimeType") or _mime_type(data)}
+            if "name" in img:
+                entry["name"] = img["name"]
+            self.img_map[i] = len(self.out.images)
+            self.out.images.append(entry)
+            self.out.image_bytes.append(bytes(data))
+        return self.img_map[i]
+
+    def texture(self, i):
+        if i not in self.tex_map:
+            src = self.reader.gltf["textures"][i]
+            tex = {k: v for k, v in src.items() if k not in ("sampler", "source", "extensions")}
+            if "sampler" in src:
+                s = src["sampler"]
+                if s not in self.smp_map:
+                    self.smp_map[s] = len(self.out.samplers)
+                    self.out.samplers.append(copy.deepcopy(self.reader.gltf["samplers"][s]))
+                tex["sampler"] = self.smp_map[s]
+            if "source" in src:
+                tex["source"] = self.image(src["source"])
+            self.tex_map[i] = len(self.out.textures)
+            self.out.textures.append(tex)
+        return self.tex_map[i]
+
+    def material(self, i) -> dict:
+        """A copy of material i with every textureInfo (`...Texture: {"index": i}`) re-indexed."""
+        def remap(obj):
+            if isinstance(obj, dict):
+                for k, v in obj.items():
+                    if k.endswith("Texture") and isinstance(v, dict) and "index" in v:
+                        v["index"] = self.texture(v["index"])
+                    remap(v)
+            elif isinstance(obj, list):
+                for v in obj:
+                    remap(v)
+
+        mat = copy.deepcopy(self.reader.gltf["materials"][i])
+        remap(mat)
+        return mat
+
+
 def _visual(reader: _Reader, prim: dict) -> Optional[GltfVisual]:
     """TEXCOORD_0, the material and what it references, re-indexed from 0; None when the primitive has neither."""
-    gltf = reader.gltf
     uv_acc = prim["attributes"].get("TEXCOORD_0")
     if uv_acc is None and "material" not in prim:
         return None
@@ -233,47 +334,31 @@ def _visual(reader: _Reader, prim: dict) -> Optional[GltfVisual]:
         vis.uv = reader.float_accessor(uv_acc).astype(np.float32)
     if "material" not in prim:
         return vis
-    vis.material = copy.deepcopy(gltf["materials"][prim["material"]])
-    tex_map, smp_map, img_map = {}, {}, {}
+    vis.material = _Collector(reader, vis).material(prim["material"])
+    return vis
 
-    def image(i):
-        if i not in img_map:
-            img = gltf["images"][i]
-            data = reader.view_bytes(img["bufferView"]) if "bufferView" in img else _read_uri(img["uri"], reader.path)
-            entry = {"mimeType": img.get("mimeType") or _mime_type(data)}
-            if "name" in img:
-                entry["name"] = img["name"]
-            img_map[i] = len(vis.images)
-            vis.images.append(entry)
-            vis.image_bytes.append(bytes(data))
-        return img_map[i]
 
-    def texture(i):
-        if i not in tex_map:
-            tex = {k: v for k, v in gltf["textures"][i].items() if k not in ("sampler", "source", "extensions")}
-            if "sampler" in gltf["textures"][i]:
-                s = gltf["textures"][i]["sampler"]
-                if s not in smp_map:
-                    smp_map[s] = len(vis.samplers)
-                    vis.samplers.append(copy.deepcopy(gltf["samplers"][s]))
-                tex["sampler"] = smp_map[s]
-            if "source" in gltf["textures"][i]:
-                tex["source"] = image(gltf["textures"][i]["source"])
-            tex_map[i] = len(vis.textures)
-            vis.textures.append(tex)
-        return tex_map[i]
-
-    def remap(obj):                       # every textureInfo (`...Texture: {"index": i}`) anywhere in the material
-        if isinstance(obj, dict):
-            for k, v in obj.items():
-                if k.endswith("Texture") and isinstance(v, dict) and "index" in v:
-                    v["index"] = texture(v["index"])
-                remap(v)
-        elif isinstance(obj, list):
-            for v in obj:
-                remap(v)
-
-    remap(vis.material)
+def _multi_visual(reader: _Reader, prims: list, n_verts: list, n_faces: list) -> GltfMultiVisual:
+    """The `GltfMultiVisual` of the included primitives `prims` with their vertex and face counts."""
+    ends_v, ends_f = np.cumsum(n_verts), np.cumsum(n_faces)
+    vis = GltfMultiVisual(vertex_ranges=np.stack([ends_v - n_verts, n_verts], 1).astype(np.int64),
+                          face_ranges=np.stack([ends_f - n_faces, n_faces], 1).astype(np.int64),
+                          has_uv=np.array(["TEXCOORD_0" in p["attributes"] for p in prims]))
+    if vis.has_uv.any():
+        vis.uv = np.zeros((int(ends_v[-1]), 2), np.float32)
+        for p, (start, count) in zip(prims, vis.vertex_ranges):
+            if "TEXCOORD_0" in p["attributes"]:
+                uv = reader.float_accessor(p["attributes"]["TEXCOORD_0"]).astype(np.float32)
+                if uv.shape != (count, 2):
+                    raise ValueError(f"{reader.path}: a TEXCOORD_0 of shape {uv.shape} on a primitive of {count} vertices")
+                vis.uv[start:start + count] = uv
+    collector, mat_map = _Collector(reader, vis), {}
+    for p in prims:
+        m = p.get("material")
+        if m is not None and m not in mat_map:
+            mat_map[m] = len(vis.materials)
+            vis.materials.append(collector.material(m))
+        vis.primitive_material.append(None if m is None else mat_map[m])
     return vis
 
 
@@ -300,7 +385,8 @@ def load_glb(path) -> Mesh:
     pipeline merges them itself (`mesh_input.merge_and_clean_mesh`) and expands its outputs back to these vertices.
 
     When the geometry is exactly one primitive with TEXCOORD_0 and/or a material, `visual` is a `GltfVisual` (UVs,
-    material, textures, samplers, image bytes); with several primitives it is None and a warning is logged.
+    material, textures, samplers, image bytes).  With several included primitives, at least one of them with TEXCOORD_0
+    or a material, it is a `GltfMultiVisual`: each primitive's vertex and face range, UVs and material.  Otherwise None.
 
     ValueError: no triangles, an extension in `extensionsRequired`, a sparse accessor, a bad GLB header or chunk layout."""
     data = Path(path).read_bytes()
@@ -309,7 +395,7 @@ def load_glb(path) -> Mesh:
     if required:
         raise ValueError(f"{path}: required glTF extension(s) not supported: {', '.join(required)}")
     reader = _Reader(gltf, binary, path)
-    verts, faces, prims, n = [], [], [], 0
+    verts, faces, prims, n, n_verts, n_faces = [], [], [], 0, [], []
     for mesh_i, world in _mesh_instances(gltf, path):
         for prim in gltf["meshes"][mesh_i]["primitives"]:
             mode = prim.get("mode", TRIANGLES)
@@ -328,6 +414,8 @@ def load_glb(path) -> Mesh:
             verts.append(pos @ world[:3, :3].T + world[:3, 3])
             faces.append(tri + n)
             prims.append(prim)
+            n_verts.append(len(pos))
+            n_faces.append(len(tri))
             n += len(pos)
     if not faces:
         raise ValueError(f"No mesh geometry found in {path}")
@@ -335,7 +423,7 @@ def load_glb(path) -> Mesh:
     if len(prims) == 1:
         visual = _visual(reader, prims[0])
     elif any("TEXCOORD_0" in p["attributes"] or "material" in p for p in prims):
-        logger.warning(f"{path}: {len(prims)} primitives; their UVs and materials are not merged, so the mesh has none")
+        visual = _multi_visual(reader, prims, np.array(n_verts), np.array(n_faces))
     return Mesh(vertices=np.concatenate(verts), faces=np.ascontiguousarray(np.concatenate(faces)), visual=visual)
 
 
@@ -386,6 +474,45 @@ class _GlbBuilder:
             gltf["images"] = [{**img, "bufferView": self.view(bytes(data))}
                               for img, data in zip(visual.images, visual.image_bytes)]
 
+    def add_primitives(self, gltf: dict, visual: GltfMultiVisual, faces: np.ndarray, per_vertex: list,
+                       targets: Optional[np.ndarray] = None, default_material: bool = True) -> list:
+        """One triangle primitive per range of `visual` (checked by the caller) -> the primitives.  Primitive p gets the
+        rows of its vertex range of every (name, array, component, type, min_max) in `per_vertex`, TEXCOORD_0 when
+        has_uv[p], its faces rebased to its range as u32 indices, its material (the default blue when it has none and
+        `default_material`) and the rows of its range of each (T, V, 3) morph target.  Materials, textures, samplers and
+        images go into `gltf`."""
+        materials, default, prims = copy.deepcopy(visual.materials), None, []
+        for p, ((v0, nv), (f0, nf)) in enumerate(zip(np.asarray(visual.vertex_ranges), np.asarray(visual.face_ranges))):
+            rows = slice(int(v0), int(v0 + nv))
+            attributes = {name: self.accessor(arr[rows], comp, type_, ARRAY_BUFFER, min_max=mm)
+                          for name, arr, comp, type_, mm in per_vertex}
+            if visual.has_uv[p]:
+                attributes["TEXCOORD_0"] = self.accessor(np.asarray(visual.uv, np.float32)[rows], F32, "VEC2", ARRAY_BUFFER)
+            prim = {"attributes": attributes,
+                    "indices": self.accessor((faces[f0:f0 + nf] - v0).reshape(-1, 1), U32, "SCALAR", ELEMENT_ARRAY_BUFFER)}
+            material = visual.primitive_material[p]
+            if material is None and default_material:
+                if default is None:
+                    default = len(materials)
+                    materials.append(copy.deepcopy(DEFAULT_MATERIAL))
+                material = default
+            if material is not None:
+                prim["material"] = int(material)
+            prim["mode"] = TRIANGLES
+            if targets is not None:
+                prim["targets"] = [{"POSITION": self.accessor(t[rows], F32, "VEC3", ARRAY_BUFFER, min_max=True)}
+                                   for t in targets]
+            prims.append(prim)
+        if materials:
+            gltf["materials"] = materials
+        for key in ("textures", "samplers"):
+            if getattr(visual, key):
+                gltf[key] = copy.deepcopy(getattr(visual, key))
+        if visual.images:
+            gltf["images"] = [{**img, "bufferView": self.view(bytes(data))}
+                              for img, data in zip(visual.images, visual.image_bytes)]
+        return prims
+
     def write(self, path, gltf: dict) -> None:
         gltf = {"asset": {"version": "2.0", "generator": "actionmesh_b200"}, **gltf}
         if self.bin:
@@ -415,12 +542,21 @@ def write_glb(path, mesh) -> None:
     """Write `mesh` (`.vertices` (V, 3), `.faces` (F, 3)) as a GLB file: one scene, one node, one mesh, one triangle
     primitive, what trimesh exports for an untextured `Trimesh(process=False)`.  POSITION is float32 with min/max, indices
     u32.  A `GltfVisual` in `mesh.visual` is written as TEXCOORD_0 plus its material, textures, samplers and images.  A
-    mesh without faces gives a scene whose one node has no mesh."""
+    `GltfMultiVisual` gives one primitive per range instead, each with its own POSITION, TEXCOORD_0 (when it has UVs),
+    rebased indices and material (none when it has none); ValueError when its ranges do not fit the mesh.  A mesh without
+    faces gives a scene whose one node has no mesh."""
     verts, faces = _mesh_arrays(mesh)
     _check_faces(faces, len(verts))
     b = _GlbBuilder()
     gltf: dict = {"scene": 0, "scenes": [{"nodes": [0]}], "nodes": [{}]}
-    if len(faces):
+    visual = getattr(mesh, "visual", None)
+    if len(faces) and isinstance(visual, GltfMultiVisual):
+        check_multi_visual(visual, len(verts), faces)
+        prims = b.add_primitives(gltf, visual, faces, [("POSITION", np.asarray(verts, np.float32), F32, "VEC3", True)],
+                                 default_material=False)
+        gltf["meshes"] = [{"primitives": prims}]
+        gltf["nodes"] = [{"mesh": 0}]
+    elif len(faces):
         attributes = {"POSITION": b.accessor(verts, F32, "VEC3", ARRAY_BUFFER, min_max=True)}
         prim = {"attributes": attributes, "indices": b.accessor(faces.reshape(-1, 1), U32, "SCALAR",
                                                                 ELEMENT_ARRAY_BUFFER), "mode": TRIANGLES}
@@ -433,7 +569,7 @@ def write_glb(path, mesh) -> None:
     b.write(path, gltf)
 
 
-def write_animated_glb(path, vertices, faces, fps: float = 8, visual: Optional[GltfVisual] = None) -> None:
+def write_animated_glb(path, vertices, faces, fps: float = 8, visual=None) -> None:
     """Write (T, V, 3) `vertices` on (F, 3) `faces` as an animated GLB: the file the reference's `create_animated_glb`
     gets from Blender, without Blender.
 
@@ -441,7 +577,8 @@ def write_animated_glb(path, vertices, faces, fps: float = 8, visual: Optional[G
     and one LINEAR `weights` animation with keyframes at k / fps whose weights are the T x T identity: frame k shows
     target k alone.  Positions are mapped by `ANIMATED_GLB_MAP` as the reference's npy + Blender export maps them: the base
     is M v_0 and target k holds M v_k - M v_0.  Without `visual` the material is the reference's default blue,
-    double-sided; with one its UVs, material and textures are kept.  No normals, no Draco: about 12 T V bytes of morph
+    double-sided; with one its UVs, material and textures are kept.  A `GltfMultiVisual` gives one primitive per range,
+    each with the T targets over its range and its own material (the default blue when it has none).  No normals, no Draco: about 12 T V bytes of morph
     data (7 MB at 31 frames x 20 000 vertices)."""
     v = np.asarray(vertices, dtype=np.float64)
     f = np.asarray(faces).reshape(-1, 3)
@@ -454,26 +591,40 @@ def write_animated_glb(path, vertices, faces, fps: float = 8, visual: Optional[G
     mapped = v @ ANIMATED_GLB_MAP.T
     base = mapped[0].astype(np.float32)
     b = _GlbBuilder()
+    gltf: dict = {"scene": 0, "scenes": [{"nodes": [0]}], "nodes": [{"mesh": 0, "name": "AnimatedMesh"}]}
+    weights = np.eye(n_frames, dtype=np.float32)
+    mesh = {"name": "AnimatedMesh", "weights": weights[0].tolist(),
+            "extras": {"targetNames": [f"Frame_{k}" for k in range(n_frames)]}}
+    if isinstance(visual, GltfMultiVisual):
+        check_multi_visual(visual, v.shape[1], f)
+        targets = (mapped - base).astype(np.float32)
+        mesh["primitives"] = b.add_primitives(gltf, visual, f, [("POSITION", base, F32, "VEC3", True)], targets)
+        gltf["meshes"] = [mesh]
+        _write_weights_animation(b, gltf, weights, fps)
+        b.write(path, gltf)
+        return
     attributes = {"POSITION": b.accessor(base, F32, "VEC3", ARRAY_BUFFER, min_max=True)}
     targets = [{"POSITION": b.accessor((mapped[k] - base).astype(np.float32), F32, "VEC3", ARRAY_BUFFER, min_max=True)}
                for k in range(n_frames)]
     indices = b.accessor(f.reshape(-1, 1), U32, "SCALAR", ELEMENT_ARRAY_BUFFER)
-    gltf: dict = {"scene": 0, "scenes": [{"nodes": [0]}], "nodes": [{"mesh": 0, "name": "AnimatedMesh"}]}
     b.add_visual(gltf, attributes, visual, v.shape[1])
     if "materials" not in gltf:
         gltf["materials"] = [copy.deepcopy(DEFAULT_MATERIAL)]
-    weights = np.eye(n_frames, dtype=np.float32)
-    gltf["meshes"] = [{"name": "AnimatedMesh", "weights": weights[0].tolist(),
-                       "extras": {"targetNames": [f"Frame_{k}" for k in range(n_frames)]},
-                       "primitives": [{"attributes": attributes, "indices": indices, "material": 0, "mode": TRIANGLES,
-                                       "targets": targets}]}]
+    mesh["primitives"] = [{"attributes": attributes, "indices": indices, "material": 0, "mode": TRIANGLES, "targets": targets}]
+    gltf["meshes"] = [mesh]
+    _write_weights_animation(b, gltf, weights, fps)
+    b.write(path, gltf)
+
+
+def _write_weights_animation(b: _GlbBuilder, gltf: dict, weights: np.ndarray, fps: float) -> None:
+    """The animated GLB's one LINEAR `weights` animation of node 0: keyframe k at k / fps holds row k of `weights`."""
+    n_frames = len(weights)
     times = b.accessor((np.arange(n_frames, dtype=np.float64) / fps).astype(np.float32).reshape(-1, 1), F32, "SCALAR",
                        min_max=True)
     gltf["animations"] = [{"name": "Animation",
                            "channels": [{"sampler": 0, "target": {"node": 0, "path": "weights"}}],
                            "samplers": [{"input": times, "output": b.accessor(weights.reshape(-1, 1), F32, "SCALAR"),
                                          "interpolation": "LINEAR"}]}]
-    b.write(path, gltf)
 
 
 def _quaternions(rot: np.ndarray) -> np.ndarray:
@@ -494,7 +645,7 @@ def _quaternions(rot: np.ndarray) -> np.ndarray:
     return q / np.linalg.norm(q, axis=-1, keepdims=True)
 
 
-def write_skinned_glb(path, fit, faces, fps: float = 8, visual: Optional[GltfVisual] = None) -> None:
+def write_skinned_glb(path, fit, faces, fps: float = 8, visual=None) -> None:
     """Write a `skinning.SkinningFit` on (F, 3) `faces` as a skinned GLB: one rest mesh, n_bones joints and one LINEAR
     animation, in the coordinates of `write_animated_glb` (DESIGN §20).
 
@@ -503,7 +654,9 @@ def write_skinned_glb(path, fit, faces, fps: float = 8, visual: Optional[GltfVis
     rest centre), with inverse bind matrix translate(-M c_j).  Keyframe k at k / fps sets joint j's rotation to the
     quaternion of M R_j^k M^T (each key's sign chosen closest to the previous key's) and its translation to
     M (R_j^k c_j + t_j^k), so that the joint matrix is M [R_j^k | t_j^k] M^T.  Without `visual` the material is the animated
-    GLB's default blue, double-sided; with one its UVs, material and textures are kept."""
+    GLB's default blue, double-sided; with one its UVs, material and textures are kept.  A `GltfMultiVisual` gives one
+    primitive per range, each with JOINTS_0 and WEIGHTS_0 over its range under the one skin and its own material (the
+    default blue when it has none)."""
     rest = np.asarray(fit.rest, dtype=np.float64)
     f = np.asarray(faces).reshape(-1, 3)
     rot, trans, centres = (np.asarray(a, dtype=np.float64) for a in (fit.rotations, fit.translations, fit.centres))
@@ -518,21 +671,26 @@ def write_skinned_glb(path, fit, faces, fps: float = 8, visual: Optional[GltfVis
     if w.shape != (len(rest), 4) or (w < 0).any() or not (total > 0).all():
         raise ValueError("weights must be (V, 4), non-negative, with a positive sum per vertex")
     M = ANIMATED_GLB_MAP
-    b = _GlbBuilder()
-    attributes = {"POSITION": b.accessor((rest @ M.T).astype(np.float32), F32, "VEC3", ARRAY_BUFFER, min_max=True),
-                  "JOINTS_0": b.accessor(np.asarray(fit.joints, dtype=np.uint8), U8, "VEC4", ARRAY_BUFFER),
-                  "WEIGHTS_0": b.accessor((w / total).astype(np.float32), F32, "VEC4", ARRAY_BUFFER)}
-    indices = b.accessor(f.reshape(-1, 1), U32, "SCALAR", ELEMENT_ARRAY_BUFFER)
     mc = centres @ M.T
     joint_nodes = list(range(2, 2 + B))
     gltf: dict = {"scene": 0, "scenes": [{"nodes": [0, 1]}],
                   "nodes": [{"mesh": 0, "skin": 0, "name": "SkinnedMesh"}, {"name": "Armature", "children": joint_nodes}]
                   + [{"name": f"Bone_{j}", "translation": mc[j].tolist()} for j in range(B)]}
-    b.add_visual(gltf, attributes, visual, len(rest))
-    if "materials" not in gltf:
-        gltf["materials"] = [copy.deepcopy(DEFAULT_MATERIAL)]
-    gltf["meshes"] = [{"name": "SkinnedMesh", "primitives": [{"attributes": attributes, "indices": indices, "material": 0,
-                                                              "mode": TRIANGLES}]}]
+    b = _GlbBuilder()
+    per_vertex = [("POSITION", (rest @ M.T).astype(np.float32), F32, "VEC3", True),
+                  ("JOINTS_0", np.asarray(fit.joints, dtype=np.uint8), U8, "VEC4", False),
+                  ("WEIGHTS_0", (w / total).astype(np.float32), F32, "VEC4", False)]
+    if isinstance(visual, GltfMultiVisual):
+        check_multi_visual(visual, len(rest), f)
+        gltf["meshes"] = [{"name": "SkinnedMesh", "primitives": b.add_primitives(gltf, visual, f, per_vertex)}]
+    else:
+        attributes = {name: b.accessor(arr, comp, type_, ARRAY_BUFFER, min_max=mm) for name, arr, comp, type_, mm in per_vertex}
+        indices = b.accessor(f.reshape(-1, 1), U32, "SCALAR", ELEMENT_ARRAY_BUFFER)
+        b.add_visual(gltf, attributes, visual, len(rest))
+        if "materials" not in gltf:
+            gltf["materials"] = [copy.deepcopy(DEFAULT_MATERIAL)]
+        gltf["meshes"] = [{"name": "SkinnedMesh", "primitives": [{"attributes": attributes, "indices": indices,
+                                                                  "material": 0, "mode": TRIANGLES}]}]
     ibm = np.tile(np.eye(4), (B, 1, 1))
     ibm[:, :3, 3] = -mc
     gltf["skins"] = [{"joints": joint_nodes, "skeleton": 1,

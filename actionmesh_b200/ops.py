@@ -11,6 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -764,16 +765,28 @@ def texture_level_table(width: int, height: int) -> list[tuple[int, int, int]]:
         w, h = max(1, w >> 1), max(1, h >> 1)
 
 
-def texture_levels(image: torch.Tensor) -> tuple[torch.Tensor, list[tuple[int, int, int]]]:
+def texture_chain_bytes(width: int, height: int) -> int:
+    """Bytes of the full mip chain of a width x height RGB texture."""
+    off, w, h = texture_level_table(width, height)[-1]
+    return off + 3 * w * h
+
+
+def texture_levels(image: torch.Tensor, out: Optional[torch.Tensor] = None,
+                   offset: int = 0) -> tuple[torch.Tensor, list[tuple[int, int, int]]]:
     """The mip chain of an (h, w, 3) uint8 CUDA image -> (levels, table): every level packed into one uint8 buffer at the
-    byte offsets of `texture_level_table`; level l + 1 averages 2 x 2 texels of level l, rounding half up."""
+    byte offsets of `texture_level_table`; level l + 1 averages 2 x 2 texels of level l, rounding half up.  With `out` (a
+    1-D uint8 buffer) the chain is written into it from byte `offset` on, and the table's offsets are absolute in it."""
     dev = _device(image, "image")
     assert image.dim() == 3 and image.shape[2] == 3 and image.dtype == torch.uint8, "image: expected (h, w, 3) uint8"
     h, w = image.shape[:2]
-    table = texture_level_table(w, h)
-    off, lw, lh = table[-1]
-    levels = torch.empty(off + 3 * lw * lh, dtype=torch.uint8, device=image.device)
-    levels[:3 * w * h].copy_(image.reshape(-1))
+    table = [(offset + off, lw, lh) for off, lw, lh in texture_level_table(w, h)]
+    if out is None:
+        assert offset == 0, "offset needs out"
+        out = torch.empty(texture_chain_bytes(w, h), dtype=torch.uint8, device=image.device)
+    assert out.dim() == 1 and out.is_contiguous() and 0 <= offset and offset + texture_chain_bytes(w, h) <= out.numel(), \
+        "out: expected a contiguous 1-D buffer holding the chain from offset on"
+    levels = out
+    levels[offset:offset + 3 * w * h].copy_(image.reshape(-1))
     _launch(_abi.amb_render_texture_levels, len(table) - 1, _ptr(levels, torch.uint8, "levels", dev),
             (C.c_int64 * (3 * len(table)))(*[x for row in table for x in row]), len(table))
     return levels, table
@@ -811,6 +824,83 @@ def shade_texture(vertices: torch.Tensor, faces: torch.Tensor, normals: torch.Te
             n_cams, float(focal), S, _ptr(pix_to_face, torch.int32, "pix_to_face", dev),
             _ptr(levels, torch.uint8, "levels", dev), table_arg, n_levels, int(mag_filter), int(min_filter), int(wrap_s),
             int(wrap_t), r, g, b, _ptr(cells, torch.uint8, "out", dev), out.stride(0), 3 * S)
+    return out
+
+
+# struct amb_shade_record of the header: a mip chain (or none), the sampler's enums and the base colour factor
+SHADE_RECORD = np.dtype({"names": ["level_offset", "level_width", "level_height", "n_levels", "mag_filter", "min_filter",
+                                   "wrap_s", "wrap_t", "base_color"],
+                         "formats": [("<i8", 15), ("<i4", 15), ("<i4", 15), "<i4", "<i4", "<i4", "<i4", "<i4", ("<f4", 3)],
+                         "offsets": [0, 120, 180, 240, 244, 248, 252, 256, 260], "itemsize": 272})
+MAX_SHADE_RECORDS = 65536
+
+
+def shade_records(records: list, levels: Optional[torch.Tensor], device) -> torch.Tensor:
+    """The shading records of `shade_materials`, checked on the host and uploaded -> (n, 272) uint8 on `device`.
+
+    Each record is (table, mag_filter, min_filter, wrap_s, wrap_t, base_color): table is None (no texture) or a chain's
+    `texture_levels` table, which must describe a full mip chain inside `levels`; the enums are glTF's."""
+    n = len(records)
+    if not 1 <= n <= MAX_SHADE_RECORDS:
+        raise _lib.AmbError(f"shade_records: {n} records; between 1 and {MAX_SHADE_RECORDS} are allowed")
+    size = 0 if levels is None else levels.numel()
+    packed = np.zeros(n, SHADE_RECORD)
+    for i, (table, mag, mn, ws, wt, base) in enumerate(records):
+        if mag not in MAG_FILTERS or mn not in MIN_FILTERS or ws not in WRAP_MODES or wt not in WRAP_MODES:
+            raise _lib.AmbError(f"shade_records: record {i} has a sampler enum glTF does not define ({mag}, {mn}, {ws}, {wt})")
+        if table is not None:
+            table = [tuple(int(x) for x in row) for row in table]
+            chain = texture_level_table(table[0][1], table[0][2])
+            if [(w, h) for _, w, h in table] != [(w, h) for _, w, h in chain] or not 1 <= min(table[0][1:]) <= max(table[0][1:]) <= 16384 \
+                    or any(b[0] < a[0] + 3 * a[1] * a[2] for a, b in zip(table, table[1:])) or table[0][0] < 0 \
+                    or table[-1][0] + 3 > size:
+                raise _lib.AmbError(f"shade_records: record {i}'s table is not a full mip chain inside the {size}-byte levels")
+            packed[i]["n_levels"] = len(table)
+            for l, (off, w, h) in enumerate(table):
+                packed[i]["level_offset"][l], packed[i]["level_width"][l], packed[i]["level_height"][l] = off, w, h
+        packed[i]["mag_filter"], packed[i]["min_filter"], packed[i]["wrap_s"], packed[i]["wrap_t"] = mag, mn, ws, wt
+        packed[i]["base_color"] = [float(x) for x in base]
+    return torch.from_numpy(packed.view(np.uint8).reshape(n, SHADE_RECORD.itemsize)).to(device)
+
+
+def face_records(face_record, n_records: int, device) -> torch.Tensor:
+    """(F,) record index per face, checked on the host to lie in [0, n_records) and uploaded -> int32 on `device`."""
+    fr = np.ascontiguousarray(np.asarray(face_record).reshape(-1))
+    if fr.dtype.kind not in "iu" or (len(fr) and (fr.min() < 0 or fr.max() >= n_records)):
+        raise _lib.AmbError(f"face_records: every entry must be an integer in [0, {n_records})")
+    return torch.from_numpy(fr.astype(np.int32)).to(device)
+
+
+def shade_materials(vertices: torch.Tensor, faces: torch.Tensor, normals: torch.Tensor, cameras: torch.Tensor, focal: float,
+                    pix_to_face: torch.Tensor, face_record: torch.Tensor, records: torch.Tensor,
+                    levels: Optional[torch.Tensor] = None, uv: Optional[torch.Tensor] = None, *,
+                    out: Optional[torch.Tensor] = None, column: int = 0) -> torch.Tensor:
+    """`shade_texture` with a shading record per face: the samples of face f shade with record face_record[f], as
+    `shade_texture` shades with that one record.  `face_record` comes from `face_records` and `records` from
+    `shade_records` (which check what the device does not); `levels` is the buffer their tables index and `uv` (V, 2)
+    fp32, both needed when a record has a texture.  Same `out` / `column` layout as `shade_normals` -> out."""
+    dev, V, F = _render_mesh(vertices, faces)
+    n_cams = _cameras(cameras)
+    assert pix_to_face.dim() == 3 and pix_to_face.shape[0] == n_cams and pix_to_face.shape[1] == pix_to_face.shape[2] \
+        and pix_to_face.shape[1] % 2 == 0 and pix_to_face.is_contiguous(), "pix_to_face: expected a contiguous (C, 2S, 2S) tensor"
+    assert normals.shape == vertices.shape and normals.is_contiguous(), "normals: expected a contiguous (V, 3) tensor"
+    assert tuple(face_record.shape) == (F,) and face_record.is_contiguous(), "face_record: expected a contiguous (F,) tensor"
+    assert records.dim() == 2 and records.shape[1] == SHADE_RECORD.itemsize and records.is_contiguous(), \
+        "records: expected a contiguous (n, 272) tensor from shade_records"
+    if uv is not None:
+        assert tuple(uv.shape) == (V, 2) and uv.is_contiguous(), "uv: expected a contiguous (V, 2) tensor"
+    S = pix_to_face.shape[1] // 2
+    if out is None:
+        out = torch.empty(S, n_cams * S, 3, dtype=torch.uint8, device=vertices.device)
+    assert out.dim() == 3 and out.shape[0] == S and out.shape[2] == 3 and out.stride(2) == 1 and out.stride(1) == 3 \
+        and 0 <= column and (column + n_cams) * S <= out.shape[1], "out: expected an (S, >= (column + C) * S, 3) row-major tensor"
+    cells = out[:, column * S:(column + n_cams) * S]
+    _launch(_abi.amb_render_shade_materials, 1, _ptr(vertices, torch.float32, "vertices", dev), V,
+            _ptr(faces, torch.int32, "faces", dev), F, _ptr(normals, torch.float32, "normals", dev),
+            _ptr(uv, torch.float32, "uv", dev), _ptr(cameras, torch.float32, "cameras", dev), n_cams, float(focal), S,
+            _ptr(pix_to_face, torch.int32, "pix_to_face", dev), _ptr(face_record, torch.int32, "face_record", dev),
+            _ptr(records, torch.uint8, "records", dev), records.shape[0], _ptr(levels, torch.uint8, "levels", dev),
+            _ptr(cells, torch.uint8, "out", dev), out.stride(0), 3 * S)
     return out
 
 

@@ -229,7 +229,8 @@ class PassThroughMeshProcess:
 @dataclass
 class Mesh:
     """Minimal mesh record returned when `trimesh` is not installed: (V, 3) float32 vertices + (F, 3) int faces (numpy).
-    `visual` is the texture side `gltf.load_glb` reads (a `gltf.GltfVisual`), or None."""
+    `visual` is the texture side `gltf.load_glb` reads: a `gltf.GltfVisual` for one primitive, a `gltf.GltfMultiVisual`
+    for several, or None."""
     vertices: "object"
     faces: "object"
     visual: "object" = None

@@ -72,6 +72,12 @@ def resample_list(items: list, target_length: int) -> list:
 def mesh_arrays(mesh) -> tuple[np.ndarray, np.ndarray]:
     """(vertices (V, 3) float32, faces (F', 3) int32) of anything with .vertices / .faces, with the faces that repeat a corner
     dropped.  Raises ValueError on a face index outside [0, V) or a non-finite vertex."""
+    verts, faces, keep = _mesh_arrays(mesh)
+    return verts, faces[keep].astype(np.int32)
+
+
+def _mesh_arrays(mesh) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """`mesh_arrays` before the drop: (vertices, every face (F, 3) int64, the faces kept (F,) bool)."""
     with np.errstate(over="ignore"):
         verts = np.asarray(mesh.vertices, dtype=np.float64).reshape(-1, 3).astype(np.float32)
     faces = np.asarray(mesh.faces, dtype=np.int64).reshape(-1, 3)
@@ -80,7 +86,7 @@ def mesh_arrays(mesh) -> tuple[np.ndarray, np.ndarray]:
     if len(faces) and (faces.min() < 0 or faces.max() >= len(verts)):
         raise ValueError(f"render: face indices must lie in [0, {len(verts)})")
     keep = (faces[:, 0] != faces[:, 1]) & (faces[:, 1] != faces[:, 2]) & (faces[:, 0] != faces[:, 2])
-    return verts, faces[keep].astype(np.int32)
+    return verts, faces, keep
 
 
 def _frame_rgb(frame, size: int) -> np.ndarray:
@@ -119,47 +125,100 @@ class TextureShading:
     base_color: tuple
 
 
-def texture_shading(visual) -> TextureShading:
-    """The base colour of a `gltf.GltfVisual` (or None) as the texture modality uses it.
+@dataclass
+class MaterialShading:
+    """What the texture modality samples for a `gltf.GltfMultiVisual`: one shading record per distinct (material, has UVs)
+    pair that a primitive has, each a `TextureShading` whose `image` is an index into `images` (or None for a flat colour),
+    the decoded images ((h, w, 3) uint8, each distinct image once) and the (F,) int32 record of every face."""
+    records: list
+    images: list
+    face_record: np.ndarray
 
-    No visual or no material: the animated GLB's default material colour.  A material: its `baseColorFactor` RGB, times
-    its `baseColorTexture` when that is usable (no `texCoord` other than 0, no textureInfo `extensions`, an image source
-    and UVs); an unusable texture is ignored with one warning.  The image is decoded by Pillow to RGB (alpha ignored).
-    Raises ValueError on an image side above 16384 or a sampler enum glTF does not define."""
-    from .gltf import DEFAULT_MATERIAL, GltfVisual
 
-    default = (ops.LINEAR, ops.LINEAR_MIPMAP_NEAREST, ops.REPEAT, ops.REPEAT)
-    if visual is not None and not isinstance(visual, GltfVisual):
-        raise ValueError(f"render: visual must be a gltf.GltfVisual, got {type(visual).__name__}")
-    if visual is None or visual.material is None:
-        return TextureShading(None, *default, tuple(DEFAULT_MATERIAL["pbrMetallicRoughness"]["baseColorFactor"][:3]))
-    pbr = visual.material.get("pbrMetallicRoughness", {})
+_DEFAULT_SAMPLER = (ops.LINEAR, ops.LINEAR_MIPMAP_NEAREST, ops.REPEAT, ops.REPEAT)
+
+
+def _record(material: Optional[dict], textures: list, samplers: list, has_uv: bool, what: str, warned: Optional[set] = None):
+    """(image source index or None, sampler enums, base colour) of one material as the texture modality uses it; an
+    unusable texture is ignored with one warning (once per `what` when `warned` collects them)."""
+    from .gltf import DEFAULT_MATERIAL
+
+    if material is None:
+        return None, _DEFAULT_SAMPLER, tuple(DEFAULT_MATERIAL["pbrMetallicRoughness"]["baseColorFactor"][:3])
+    pbr = material.get("pbrMetallicRoughness", {})
     base = tuple(float(x) for x in pbr.get("baseColorFactor", [1.0, 1.0, 1.0, 1.0])[:3])
     info = pbr.get("baseColorTexture")
     if info is None:
-        return TextureShading(None, *default, base)
-    tex = visual.textures[info["index"]] if 0 <= info.get("index", -1) < len(visual.textures) else {}
+        return None, _DEFAULT_SAMPLER, base
+    tex = textures[info["index"]] if 0 <= info.get("index", -1) < len(textures) else {}
     why = ("it uses texCoord %s" % info["texCoord"] if info.get("texCoord", 0) != 0 else
            "its textureInfo has extensions (%s)" % ", ".join(info["extensions"]) if info.get("extensions") else
            "it has no image source" if "source" not in tex else
-           "the mesh has no UVs" if visual.uv is None else None)
+           "the mesh has no UVs" if not has_uv else None)
     if why is not None:
-        logger.warning(f"render: the base colour texture is ignored because {why}; shading with the base colour factor")
-        return TextureShading(None, *default, base)
-    smp = visual.samplers[tex["sampler"]] if "sampler" in tex else {}
-    mode = (smp.get("magFilter", default[0]), smp.get("minFilter", default[1]), smp.get("wrapS", default[2]),
-            smp.get("wrapT", default[3]))
+        if warned is None or what not in warned:
+            logger.warning(f"render: {what} is ignored because {why}; shading with the base colour factor")
+            if warned is not None:
+                warned.add(what)
+        return None, _DEFAULT_SAMPLER, base
+    smp = samplers[tex["sampler"]] if "sampler" in tex else {}
+    mode = (smp.get("magFilter", _DEFAULT_SAMPLER[0]), smp.get("minFilter", _DEFAULT_SAMPLER[1]),
+            smp.get("wrapS", _DEFAULT_SAMPLER[2]), smp.get("wrapT", _DEFAULT_SAMPLER[3]))
     for value, allowed, name in zip(mode, (ops.MAG_FILTERS, ops.MIN_FILTERS, ops.WRAP_MODES, ops.WRAP_MODES),
                                     ("magFilter", "minFilter", "wrapS", "wrapT")):
         if value not in allowed:
             raise ValueError(f"render: sampler {name} {value} is not a glTF value ({', '.join(map(str, allowed))})")
+    return tex["source"], mode, base
+
+
+def _decode(data: bytes) -> np.ndarray:
     from PIL import Image
 
-    with Image.open(io.BytesIO(visual.image_bytes[tex["source"]])) as img:
+    with Image.open(io.BytesIO(data)) as img:
         if max(img.size) > MAX_TEXTURE_SIDE:
             raise ValueError(f"render: texture of {img.size[0]} x {img.size[1]} texels; each side must be <= {MAX_TEXTURE_SIDE}")
-        rgb = np.array(img.convert("RGB"))
-    return TextureShading(rgb, *mode, base)
+        return np.array(img.convert("RGB"))
+
+
+def texture_shading(visual):
+    """The base colour of a `gltf.GltfVisual` (or None) as the texture modality uses it -> a `TextureShading`; of a
+    `gltf.GltfMultiVisual` -> a `MaterialShading`.
+
+    No visual or no material: the animated GLB's default material colour.  A material: its `baseColorFactor` RGB, times
+    its `baseColorTexture` when that is usable (no `texCoord` other than 0, no textureInfo `extensions`, an image source
+    and UVs); an unusable texture is ignored with one warning (per material for a multi-primitive visual).  Images are
+    decoded by Pillow to RGB (alpha ignored), each once.  Raises ValueError on an image side above 16384 or a sampler enum
+    glTF does not define."""
+    from .gltf import GltfMultiVisual, GltfVisual
+
+    if isinstance(visual, GltfMultiVisual):
+        return _material_shading(visual)
+    if visual is not None and not isinstance(visual, GltfVisual):
+        raise ValueError(f"render: visual must be a gltf.GltfVisual or gltf.GltfMultiVisual, got {type(visual).__name__}")
+    visual = GltfVisual() if visual is None else visual
+    source, mode, base = _record(visual.material, visual.textures, visual.samplers, visual.uv is not None,
+                                 "the base colour texture")
+    return TextureShading(None if source is None else _decode(visual.image_bytes[source]), *mode, base)
+
+
+def _material_shading(visual) -> MaterialShading:
+    """`texture_shading` of a `gltf.GltfMultiVisual`: records keyed by (material, has UVs) in first-use order."""
+    keys, records, images, image_of, warned = {}, [], [], {}, set()
+    prim_record = []
+    for m, has_uv in zip(visual.primitive_material, np.asarray(visual.has_uv, bool)):
+        key = (m, bool(has_uv))
+        if key not in keys:
+            material = None if m is None else visual.materials[m]
+            source, mode, base = _record(material, visual.textures, visual.samplers, key[1],
+                                         f"material {m}'s base colour texture", warned)
+            if source is not None and source not in image_of:
+                image_of[source] = len(images)
+                images.append(_decode(visual.image_bytes[source]))
+            keys[key] = len(records)
+            records.append(TextureShading(None if source is None else image_of[source], *mode, base))
+        prim_record.append(keys[key])
+    counts = np.asarray(visual.face_ranges, np.int64).reshape(-1, 2)[:, 1]
+    return MaterialShading(records, images, np.repeat(np.asarray(prim_record, np.int32), counts))
 
 
 def _modalities(modalities) -> tuple:
@@ -191,10 +250,20 @@ class B200MeshVisualizer:
     def render_frames(self, meshes: list, input_frames: Optional[list] = None, *, modalities=("normal",), visual=None):
         """The video's frames before encoding, per modality: host uint8 (n_frames, S, n_cols * S, 3), n_cols = cameras (+ 1
         for the input frame column when `input_frames` is given).  One modality -> its grid; several -> a tuple of grids in
-        the order given.  `visual` (a `gltf.GltfVisual`, its uv one row per mesh vertex) gives "texture" its base colour."""
+        the order given.  `visual` (a `gltf.GltfVisual`, its uv one row per mesh vertex) gives "texture" its base colour; a
+        `gltf.GltfMultiVisual`, whose ranges must fit every mesh, gives each face its primitive's material."""
+        from .gltf import GltfMultiVisual, check_multi_visual
+
         mods = _modalities(modalities)
         S, n = self.image_size, len(meshes)
-        arrays = [mesh_arrays(m) for m in meshes]
+        full = [_mesh_arrays(m) for m in meshes]
+        arrays = [(verts, faces[keep].astype(np.int32)) for verts, faces, keep in full]
+        if isinstance(visual, GltfMultiVisual):
+            for verts, faces, _ in full:
+                try:
+                    check_multi_visual(visual, len(verts), faces)
+                except ValueError as exc:
+                    raise ValueError(f"render: {exc}") from None
         uv = None if visual is None or getattr(visual, "uv", None) is None else np.asarray(visual.uv, dtype=np.float32)
         if uv is not None:
             if not np.isfinite(uv).all():
@@ -213,8 +282,10 @@ class B200MeshVisualizer:
         with torch.cuda.device(self.device):
             cams, focal = self._camera_table()
             grids = [torch.empty(n, S, n_cols * S, 3, dtype=torch.uint8, device=self.device) for _ in mods]
-            tex = {}
-            if shading is not None:
+            tex, face_record = {}, None
+            if isinstance(shading, MaterialShading):
+                tex = self._material_tables(shading, uv)
+            elif shading is not None:
                 tex = dict(mag_filter=shading.mag_filter, min_filter=shading.min_filter, wrap_s=shading.wrap_s,
                            wrap_t=shading.wrap_t, base_color=shading.base_color)
                 if shading.image is not None:  # the mip chain is built once per call
@@ -227,6 +298,12 @@ class B200MeshVisualizer:
                 for grid, mod in zip(grids, mods):
                     if mod == "normal":
                         ops.shade_normals(v, f, normals, cams, focal, pix_to_face, out=grid[k], column=col0)
+                    elif isinstance(shading, MaterialShading):
+                        kept = shading.face_record[full[k][2]]
+                        if face_record is None or not np.array_equal(kept, face_record[0]):  # meshes usually share faces
+                            face_record = (kept, ops.face_records(kept, len(shading.records), self.device))
+                        ops.shade_materials(v, f, normals, cams, focal, pix_to_face, face_record[1], out=grid[k],
+                                            column=col0, **tex)
                     else:
                         ops.shade_texture(v, f, normals, cams, focal, pix_to_face, out=grid[k], column=col0, **tex)
             grids = [g.cpu() for g in grids]
@@ -236,6 +313,21 @@ class B200MeshVisualizer:
                 for grid in grids:
                     grid[k, :, :S] = cell
         return grids[0] if len(grids) == 1 else tuple(grids)
+
+    def _material_tables(self, shading: MaterialShading, uv: Optional[np.ndarray]) -> dict:
+        """`shade_materials`' records, levels and uv on the device: every distinct image's mip chain built once, all of
+        them packed into one level buffer."""
+        sizes = [ops.texture_chain_bytes(img.shape[1], img.shape[0]) for img in shading.images]
+        levels = torch.empty(max(sum(sizes), 1), dtype=torch.uint8, device=self.device) if sizes else None
+        tables, off = [], 0
+        for img, size in zip(shading.images, sizes):
+            tables.append(ops.texture_levels(torch.from_numpy(img).to(self.device), out=levels, offset=off)[1])
+            off += size
+        rows = [(None if r.image is None else tables[r.image], r.mag_filter, r.min_filter, r.wrap_s, r.wrap_t, r.base_color)
+                for r in shading.records]
+        textured = any(r.image is not None for r in shading.records)
+        return dict(records=ops.shade_records(rows, levels, self.device), levels=levels,
+                    uv=torch.from_numpy(uv).to(self.device) if textured else None)
 
     @torch.no_grad()
     def render(self, meshes: list, device=None, output_dir: str = ".", input_frames: Optional[list] = None, *,

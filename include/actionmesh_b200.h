@@ -383,7 +383,23 @@ int amb_render_shade_normals(const float* vertices, int64_t n_vertices, const in
  *    mag_filter is 9728 (NEAREST) or 9729 (LINEAR); min_filter one of 9728, 9729 and 9984..9987 (*_MIPMAP_LINEAR behaves as
  *    *_MIPMAP_NEAREST); wrap_s / wrap_t are 10497 (REPEAT), 33071 (CLAMP_TO_EDGE) or 33648 (MIRRORED_REPEAT).  base_r/g/b
  *    is the material's base colour factor.  n_levels = 0 shades without a texture (colour = base factor times the
- *    headlight); levels, level_table and uv may then be NULL.  With zero faces every cell is white. */
+ *    headlight); levels, level_table and uv may then be NULL.  With zero faces every cell is white.
+ *  render_shade_materials: render_shade_texture with a shading record per face: the samples of face f shade with
+ *    records[face_record[f]], under render_shade_texture's contract for that one record (its level 0 size sets the level of
+ *    detail).  face_record: (F,) int32 DEVICE array; records: n_records struct amb_shade_record, a DEVICE array; levels: one
+ *    DEVICE buffer holding every record's chain at the record's absolute byte offsets.  Preconditions, like face indices
+ *    below V, not checked on the device: face_record entries lie in [0, n_records); each record with n_levels > 0 holds a
+ *    full chain as render_shade_texture's table describes it, inside the levels buffer, and valid sampler enums; uv and
+ *    levels are non-NULL when a record has a texture.  The entry point checks pointers, sizes, strides and
+ *    1 <= n_records <= 65536, and neither synchronises nor copies. */
+struct amb_shade_record {
+  int64_t level_offset[15]; /* byte offset of level l in the levels buffer */
+  int32_t level_width[15];
+  int32_t level_height[15];
+  int32_t n_levels;         /* 0: no texture (the base colour factor times the headlight) */
+  int32_t mag_filter, min_filter, wrap_s, wrap_t;
+  float base_color[3];
+};
 int amb_render_texture_levels(uint8_t* levels, const int64_t* level_table, int n_levels, amb_stream_t stream);
 int amb_render_shade_texture(const float* vertices, int64_t n_vertices, const int32_t* faces, int64_t n_faces,
                              const float* normals, const float* uv, const float* cameras, int n_cameras, float focal,
@@ -391,6 +407,11 @@ int amb_render_shade_texture(const float* vertices, int64_t n_vertices, const in
                              int n_levels, int mag_filter, int min_filter, int wrap_s, int wrap_t, float base_r,
                              float base_g, float base_b, uint8_t* out, int64_t row_stride, int64_t view_stride,
                              amb_stream_t stream);
+int amb_render_shade_materials(const float* vertices, int64_t n_vertices, const int32_t* faces, int64_t n_faces,
+                               const float* normals, const float* uv, const float* cameras, int n_cameras, float focal,
+                               int image_size, const int32_t* pix_to_face, const int32_t* face_record,
+                               const void* records, int n_records, const uint8_t* levels, uint8_t* out,
+                               int64_t row_stride, int64_t view_stride, amb_stream_t stream);
 
 /* ---- background removal: RMBG-1.4 around split-bf16 GEMM convolutions, mask head and refinement (csrc/rmbg.cu) -------------
  * Replaces BackgroundRemover.forward (actionmesh/preprocessing/background_removal.py:84-112) with BriaRMBG

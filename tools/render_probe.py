@@ -2,9 +2,11 @@
 grid download) with CUDA events, on a depth-9 Stage 0 mesh (~1.75 M faces, the rippled ball the geometry tests refine) and
 on that mesh decimated to 40 000 faces, at 16 and 31 frames x 3 cameras x S = 256.  Then the texture modality on the
 decimated mesh: normal only against normal + texture (a --texture-size square JPEG, decoded and mip-mapped in every call,
-on spherical UVs), the two alternated.  Prints the card and its power limit with the numbers.
+on spherical UVs), the two alternated.  Then per-face materials: the decimated mesh split into 8 primitives with 8
+distinct --texture-size JPEGs against the same split mesh with one texture, normal + texture, the two alternated.  Prints
+the card and its power limit with the numbers.
 
-    python tools/render_probe.py [--repeats 3] [--texture-size 2048]
+    python tools/render_probe.py [--repeats 3] [--texture-size 2048] [--materials-only]
 """
 import io
 import argparse
@@ -38,6 +40,7 @@ def main() -> None:
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--image-size", type=int, default=256)
     ap.add_argument("--texture-size", type=int, default=2048)
+    ap.add_argument("--materials-only", action="store_true", help="Only the per-face material comparison.")
     args = ap.parse_args()
 
     import geometry_exact as gx
@@ -58,7 +61,7 @@ def main() -> None:
     meshes = {"depth-9": (base, faces), "decimated": (np.asarray(small.vertices), np.asarray(small.faces))}
     vis = B200MeshVisualizer(image_size=args.image_size)
     for name, (v, f) in meshes.items():
-        for n in (16, 31):
+        for n in (16, 31) if not args.materials_only else ():
             clip = _frames(v, f, n)
             vis.render_frames(clip[:2])  # warm-up
             times = []
@@ -76,7 +79,7 @@ def main() -> None:
 
     v, f = meshes["decimated"]
     visual = _textured(v, args.texture_size)
-    for n in (16, 31):
+    for n in (16, 31) if not args.materials_only else ():
         clip = _frames(v, f, n)
         runs = {("normal",): [], ("normal", "texture"): []}
         for mods in runs:
@@ -91,6 +94,38 @@ def main() -> None:
                   f"(min {min(times):.1f}, max {max(times):.1f})")
 
 
+    from test_multi_material_cpu import split
+
+    groups = np.array_split(np.arange(len(f)), 8)
+    sv, sf, suv, vr, fr = split(v, f, _textured(v, 1).uv, groups)
+    one, eight = _textured(sv, args.texture_size), _materials(sv, suv, vr, fr, args.texture_size)
+    for n in (16, 31):
+        clip = _frames(sv, sf, n)
+        runs = {"1 texture": (one, []), "8 primitives, 8 textures": (eight, [])}
+        for visual, _ in runs.values():
+            vis.render_frames(clip[:2], modalities=("normal", "texture"), visual=visual)  # warm-up
+        for _ in range(args.repeats):
+            for visual, times in runs.values():
+                times.append(_timed(lambda: vis.render_frames(clip, modalities=("normal", "texture"), visual=visual)))
+        for name, (_, times) in runs.items():
+            ms = float(np.median(times))
+            print(f"split decimated: {len(sf):,} faces, {n} frames x 3 views, S = {args.image_size}, normal + texture, "
+                  f"{name} of {args.texture_size}^2: {ms:.1f} ms per clip (min {min(times):.1f}, max {max(times):.1f})")
+
+
+def _materials(v, uv, vertex_ranges, face_ranges, size: int):
+    """A GltfMultiVisual: primitive p has material p with its own size x size JPEG (seeded per primitive)."""
+    from actionmesh_b200.gltf import GltfMultiVisual
+
+    P = len(vertex_ranges)
+    jpegs = [_jpeg(size, seed) for seed in range(1, P + 1)]
+    return GltfMultiVisual(vertex_ranges=vertex_ranges, face_ranges=face_ranges, uv=uv, has_uv=np.ones(P, bool),
+                           primitive_material=list(range(P)),
+                           materials=[{"pbrMetallicRoughness": {"baseColorTexture": {"index": p}}} for p in range(P)],
+                           textures=[{"source": p} for p in range(P)], images=[{"mimeType": "image/jpeg"}] * P,
+                           image_bytes=jpegs)
+
+
 def _timed(fn) -> float:
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     torch.cuda.synchronize()
@@ -103,20 +138,25 @@ def _timed(fn) -> float:
 
 def _textured(v: np.ndarray, size: int):
     """A GltfVisual on spherical UVs with a size x size JPEG: a colour gradient with seeded noise."""
-    from PIL import Image
-
     from actionmesh_b200.gltf import GltfVisual
 
     c = v - v.mean(0)
     uv = np.stack([np.arctan2(c[:, 2], c[:, 0]) / (2 * np.pi) + 0.5,
                    np.arccos(np.clip(c[:, 1] / np.linalg.norm(c, axis=1), -1, 1)) / np.pi], 1).astype(np.float32)
+    return GltfVisual(uv=uv, material={"pbrMetallicRoughness": {"baseColorTexture": {"index": 0}}},
+                      textures=[{"source": 0}], images=[{"mimeType": "image/jpeg"}], image_bytes=[_jpeg(size, 0)])
+
+
+def _jpeg(size: int, seed: int) -> bytes:
+    """A size x size JPEG: a colour gradient with seeded noise."""
+    from PIL import Image
+
     y, x = np.mgrid[0:size, 0:size]
-    noise = np.random.default_rng(0).integers(0, 48, (size, size, 3))
+    noise = np.random.default_rng(seed).integers(0, 48, (size, size, 3))
     img = np.stack([x * 200 // size, y * 200 // size, (x + y) * 100 // size], -1) + noise
     buf = io.BytesIO()
     Image.fromarray(img.astype(np.uint8)).save(buf, format="JPEG", quality=90)
-    return GltfVisual(uv=uv, material={"pbrMetallicRoughness": {"baseColorTexture": {"index": 0}}},
-                      textures=[{"source": 0}], images=[{"mimeType": "image/jpeg"}], image_bytes=[buf.getvalue()])
+    return buf.getvalue()
 
 
 if __name__ == "__main__":
