@@ -5,6 +5,8 @@
   write_glb(path, mesh)                      one node, one mesh, one triangle primitive per material (what trimesh exports)
   write_animated_glb(path, vertices, faces)  one morph target per frame and a weights animation (what Blender exports)
   write_skinned_glb(path, fit, faces)        a rest mesh, its bones and skin weights, and a joint animation
+  load_rig(path) -> GltfRig                  a rigged file's skeleton and skin, in load_glb's vertex order
+  write_rig_animation(src, out, rig, fit)    the source file plus one joint animation (DESIGN.md §21)
   save_meshes(meshes, output_dir)            mesh_00.glb, mesh_01.glb, ...
   save_deformation(meshes, path)             {stem}_vertices.npy / {stem}_faces.npy
 
@@ -36,7 +38,7 @@ ARRAY_BUFFER, ELEMENT_ARRAY_BUFFER = 34962, 34963
 F32, U8, U16, U32 = 5126, 5121, 5123, 5125
 COMPONENT_DTYPES = {5120: np.dtype("<i1"), U8: np.dtype("<u1"), 5122: np.dtype("<i2"), U16: np.dtype("<u2"),
                     U32: np.dtype("<u4"), F32: np.dtype("<f4")}
-TYPE_SIZES = {"SCALAR": 1, "VEC2": 2, "VEC3": 3, "VEC4": 4}
+TYPE_SIZES = {"SCALAR": 1, "VEC2": 2, "VEC3": 3, "VEC4": 4, "MAT4": 16}
 TRIANGLES, TRIANGLE_STRIP, TRIANGLE_FAN = 4, 5, 6
 
 # (x, y, z) -> (-z, y, -x): `save_deformation`'s (x, y, z) -> (-z, x, y) followed by Blender's +Y-up export
@@ -252,21 +254,24 @@ def _root_nodes(gltf: dict) -> list:
     return [i for i in range(len(gltf.get("nodes", []))) if i not in children]
 
 
-def _mesh_instances(gltf: dict, path) -> list:
-    """[(mesh index, 4x4 world transform)] in depth-first node order, children in their listed order."""
+def _mesh_instances(gltf: dict, path, visited: Optional[dict] = None) -> list:
+    """[(mesh index, 4x4 world transform, node index)] in depth-first node order, children in their listed order.  When
+    `visited` is a dict it receives node -> (parent node or -1, world transform) for every node reached."""
     nodes, out = gltf.get("nodes", []), []
 
-    def visit(i, parent, ancestors):
+    def visit(i, parent_i, parent, ancestors):
         if i in ancestors:
             raise ValueError(f"{path}: node {i} is its own ancestor")
         world = parent @ _node_matrix(nodes[i])
+        if visited is not None:
+            visited[i] = (parent_i, world)
         if "mesh" in nodes[i]:
-            out.append((nodes[i]["mesh"], world))
+            out.append((nodes[i]["mesh"], world, i))
         for c in nodes[i].get("children", []):
-            visit(c, world, ancestors | {i})
+            visit(c, i, world, ancestors | {i})
 
     for r in _root_nodes(gltf):
-        visit(r, np.eye(4), frozenset())
+        visit(r, -1, np.eye(4), frozenset())
     return out
 
 
@@ -372,6 +377,41 @@ def _mime_type(data: bytes) -> str:
     raise ValueError("image of unknown type (neither PNG, JPEG nor WebP)")
 
 
+@dataclass
+class _Primitive:
+    """One primitive `load_glb` includes: its mesh, node, node world matrix and JSON, POSITION as stored (float64), the
+    vertices in world space and its triangles (reversed where the world matrix mirrors)."""
+    mesh: int
+    node: int
+    world: np.ndarray
+    prim: dict
+    positions: np.ndarray
+    vertices: np.ndarray
+    triangles: np.ndarray
+
+
+def _included_primitives(gltf: dict, reader: _Reader, path, visited: Optional[dict] = None) -> list:
+    """The triangle primitives `load_glb` includes, in its order (`visited` as in `_mesh_instances`)."""
+    out = []
+    for mesh_i, world, node in _mesh_instances(gltf, path, visited):
+        for prim in gltf["meshes"][mesh_i]["primitives"]:
+            mode = prim.get("mode", TRIANGLES)
+            if mode not in (TRIANGLES, TRIANGLE_STRIP, TRIANGLE_FAN) or "POSITION" not in prim["attributes"]:
+                continue
+            pos = reader.float_accessor(prim["attributes"]["POSITION"])
+            idx = (reader.accessor(prim["indices"])[:, 0].astype(np.int64) if "indices" in prim
+                   else np.arange(len(pos), dtype=np.int64))
+            if len(idx) and (idx.min() < 0 or idx.max() >= len(pos)):
+                raise ValueError(f"{path}: mesh {mesh_i} has an index outside its {len(pos)} vertices")
+            tri = _triangles(idx, mode)
+            if not len(tri):
+                continue
+            if np.linalg.det(world[:3, :3]) < 0:
+                tri = tri[:, ::-1]
+            out.append(_Primitive(mesh_i, node, world, prim, pos, pos @ world[:3, :3].T + world[:3, 3], tri))
+    return out
+
+
 def load_glb(path) -> Mesh:
     """Read a .glb file into one `Mesh`: the reference's `load_glb` (trimesh `load(..., force="mesh")`).
 
@@ -395,28 +435,15 @@ def load_glb(path) -> Mesh:
     if required:
         raise ValueError(f"{path}: required glTF extension(s) not supported: {', '.join(required)}")
     reader = _Reader(gltf, binary, path)
+    included = _included_primitives(gltf, reader, path)
     verts, faces, prims, n, n_verts, n_faces = [], [], [], 0, [], []
-    for mesh_i, world in _mesh_instances(gltf, path):
-        for prim in gltf["meshes"][mesh_i]["primitives"]:
-            mode = prim.get("mode", TRIANGLES)
-            if mode not in (TRIANGLES, TRIANGLE_STRIP, TRIANGLE_FAN) or "POSITION" not in prim["attributes"]:
-                continue
-            pos = reader.float_accessor(prim["attributes"]["POSITION"])
-            idx = (reader.accessor(prim["indices"])[:, 0].astype(np.int64) if "indices" in prim
-                   else np.arange(len(pos), dtype=np.int64))
-            if len(idx) and (idx.min() < 0 or idx.max() >= len(pos)):
-                raise ValueError(f"{path}: mesh {mesh_i} has an index outside its {len(pos)} vertices")
-            tri = _triangles(idx, mode)
-            if not len(tri):
-                continue
-            if np.linalg.det(world[:3, :3]) < 0:
-                tri = tri[:, ::-1]
-            verts.append(pos @ world[:3, :3].T + world[:3, 3])
-            faces.append(tri + n)
-            prims.append(prim)
-            n_verts.append(len(pos))
-            n_faces.append(len(tri))
-            n += len(pos)
+    for p in included:
+        verts.append(p.vertices)
+        faces.append(p.triangles + n)
+        prims.append(p.prim)
+        n_verts.append(len(p.vertices))
+        n_faces.append(len(p.triangles))
+        n += len(p.vertices)
     if not faces:
         raise ValueError(f"No mesh geometry found in {path}")
     visual = None
@@ -425,6 +452,242 @@ def load_glb(path) -> Mesh:
     elif any("TEXCOORD_0" in p["attributes"] or "material" in p for p in prims):
         visual = _multi_visual(reader, prims, np.array(n_verts), np.array(n_faces))
     return Mesh(vertices=np.concatenate(verts), faces=np.ascontiguousarray(np.concatenate(faces)), visual=visual)
+
+
+# --------------------------------------------------------------------------------------------------------------- the rig
+MAX_RIG_JOINTS = 1024
+MAX_INFLUENCES = 8
+RIG_TOLERANCE = 1e-6         # a parent's world matrix is a rotation times a uniform scale to this relative tolerance
+BIND_TOLERANCE = 1e-5        # the default pose reproduces the rest vertices to this fraction of the bounding-box diagonal
+
+
+@dataclass
+class GltfRig:
+    """The skeleton and skin of a rigged GLB, as `load_rig` reads them (DESIGN.md §21).  Joints are in the skin's order.
+
+    joint_nodes: (J,) the joints' node indices; parent: (J,) int64, the parent joint or -1; order: (J,) a topological
+    order (depth-first from the roots, parents first, siblings in skin order); translation / rotation (x, y, z, w) / scale:
+    (J, 3) / (J, 4) / (J, 3) fp64, each joint's default local TRS; from_matrix: (J,) bool, joints stored as `matrix`;
+    above: (J, 4, 4), the fixed world matrix above each root joint (identity for the others); inverse_bind: (J, 4, 4).
+    rest: (V, 3), `load_glb(path).vertices`; points: (V, 3), the positions the binds act on (POSITION for skinned and
+    rigid-child vertices, rest for static ones); binds: (NB, 4, 4), the J inverse bind matrices then one effective bind
+    (G_k^0)^-1 NodeWorld^0 per rigid-child node; bind_joint: (NB,); slot_bind (V, 8) int32 and slot_weight (V, 8) fp64, used
+    slots (weight > 0) first, each row summing to 1 (all zero for a static vertex)."""
+    joint_nodes: list
+    parent: np.ndarray
+    order: np.ndarray
+    translation: np.ndarray
+    rotation: np.ndarray
+    scale: np.ndarray
+    from_matrix: np.ndarray
+    above: np.ndarray
+    inverse_bind: np.ndarray
+    rest: np.ndarray
+    points: np.ndarray
+    binds: np.ndarray
+    bind_joint: np.ndarray
+    slot_bind: np.ndarray
+    slot_weight: np.ndarray
+
+
+def _similarity_scale(m: np.ndarray) -> Optional[float]:
+    """s when the 3x3 `m` is a rotation times the positive uniform scale s (to RIG_TOLERANCE), else None."""
+    g = m.T @ m
+    s2 = np.trace(g) / 3
+    if not s2 > 0 or np.linalg.det(m) <= 0 or np.abs(g - s2 * np.eye(3)).max() > RIG_TOLERANCE * s2:
+        return None
+    return float(np.sqrt(s2))
+
+
+def _trs(node: dict, path, name: str) -> tuple:
+    """A node's local (translation, rotation (x, y, z, w) unit, scale); a `matrix` is decomposed, ValueError on shear or a
+    non-positive scale."""
+    if "matrix" not in node:
+        q = np.asarray(node.get("rotation", [0.0, 0.0, 0.0, 1.0]), np.float64)
+        n = np.linalg.norm(q)
+        return (np.asarray(node.get("translation", [0.0, 0.0, 0.0]), np.float64),
+                q / n if n > 0 else np.array([0.0, 0.0, 0.0, 1.0]), np.asarray(node.get("scale", [1.0, 1.0, 1.0]), np.float64))
+    m = _node_matrix(node)
+    if np.abs(m[3] - [0, 0, 0, 1]).max() > 0:
+        raise ValueError(f"{path}: {name}'s matrix is not affine")
+    lin = m[:3, :3]
+    scale = np.linalg.norm(lin, axis=0)
+    if np.linalg.det(lin) <= 0 or not (scale > 0).all():
+        raise ValueError(f"{path}: {name}'s matrix has a non-positive scale")
+    rot = lin / scale
+    if np.abs(rot.T @ rot - np.eye(3)).max() > RIG_TOLERANCE:
+        raise ValueError(f"{path}: {name}'s matrix has shear")
+    return m[:3, 3].copy(), _quaternions(rot), scale
+
+
+def load_rig(path) -> GltfRig:
+    """Read the skeleton and skin of a rigged .glb, with the vertices in `load_glb`'s order -> GltfRig.
+
+    The file is traversed as `load_glb` traverses it.  A skinned primitive's slots come from JOINTS_0/1 (u8 or u16) and
+    WEIGHTS_0/1 (float, or normalized u8/u16), each row divided by its fp64 sum, weight-0 slots unused.  A primitive
+    without a skin whose node is, or is under, a joint follows its nearest such joint k rigidly (weight 1, bind
+    (G_k^0)^-1 NodeWorld^0); any other primitive is static.
+
+    ValueError, saying why: no skin; two distinct skins among the included nodes; a skinned mesh instanced by two nodes;
+    more than 1024 joints, a joint outside the default scene or a non-joint node between two joints; a joint `matrix` with
+    shear or a non-positive scale; a joint whose parent's default world matrix is not a rotation times a positive uniform
+    scale; more than 8 influences per vertex, a row of weights summing to 0 or a used slot's joint outside the skin; morph
+    targets with non-zero default weights on a skinned mesh; a buffer that is an external file, or no BIN chunk; a
+    default pose that moves a vertex by more than 1e-5 of the rest bounding-box diagonal (glTF skins ignore the skinned
+    node's transform, `load_glb` applies it)."""
+    data = Path(path).read_bytes()
+    gltf, binary = _parse_glb(data, path)
+    required = gltf.get("extensionsRequired") or []
+    if required:
+        raise ValueError(f"{path}: required glTF extension(s) not supported: {', '.join(required)}")
+    buffers = gltf.get("buffers") or []
+    if binary is None or not buffers or "uri" in buffers[0]:
+        raise ValueError(f"{path}: a rig is read from a GLB whose buffer 0 is its BIN chunk")
+    if any(not str(b.get("uri", "data:")).startswith("data:") for b in buffers):
+        raise ValueError(f"{path}: a buffer is an external file")
+    reader = _Reader(gltf, binary, path)
+    visited: dict = {}
+    included = _included_primitives(gltf, reader, path, visited)
+    if not included:
+        raise ValueError(f"No mesh geometry found in {path}")
+    nodes = gltf.get("nodes", [])
+    skins = sorted({nodes[p.node]["skin"] for p in included if "skin" in nodes[p.node]})
+    if not skins:
+        raise ValueError(f"{path}: no included mesh node has a skin")
+    if len(skins) > 1:
+        raise ValueError(f"{path}: the included nodes use {len(skins)} distinct skins {skins}; one is supported")
+    skin = gltf["skins"][skins[0]]
+    instances = {}
+    for mesh_i, _, node in _mesh_instances(gltf, path):
+        instances.setdefault(mesh_i, set()).add(node)
+    for p in included:
+        if "skin" in nodes[p.node] and len(instances[p.mesh]) > 1:
+            raise ValueError(f"{path}: skinned mesh {p.mesh} is instanced by {len(instances[p.mesh])} nodes")
+
+    joint_nodes = [int(n) for n in skin["joints"]]
+    J = len(joint_nodes)
+    if not 1 <= J <= MAX_RIG_JOINTS or len(set(joint_nodes)) != J:
+        raise ValueError(f"{path}: the skin has {J} joints (distinct, between 1 and {MAX_RIG_JOINTS} supported)")
+    index = {n: j for j, n in enumerate(joint_nodes)}
+    for n in joint_nodes:
+        if n not in visited:
+            raise ValueError(f"{path}: joint node {n} is not in the default scene")
+
+    def joint_ancestor(n):
+        """(nearest joint among n's strict ancestors or -1, the node directly above n)"""
+        up = visited[n][0]
+        while up >= 0 and up not in index:
+            up = visited[up][0]
+        return (index[up] if up >= 0 else -1), visited[n][0]
+
+    parent = np.full(J, -1, np.int64)
+    above = np.tile(np.eye(4), (J, 1, 1))
+    for j, n in enumerate(joint_nodes):
+        k, direct = joint_ancestor(n)
+        if k >= 0 and direct != joint_nodes[k]:
+            raise ValueError(f"{path}: non-joint node {direct} lies between joints {joint_nodes[k]} and {n}")
+        parent[j] = k
+        if k < 0 and direct >= 0:
+            above[j] = visited[direct][1]
+    trs = [_trs(nodes[n], path, f"joint node {n}") for n in joint_nodes]
+    translation = np.stack([t[0] for t in trs])
+    rotation = np.stack([t[1] for t in trs])
+    scale = np.stack([t[2] for t in trs])
+    world0 = np.stack([visited[n][1] for n in joint_nodes])
+    for j in range(J):
+        pw = world0[parent[j]] if parent[j] >= 0 else above[j]
+        if _similarity_scale(pw[:3, :3]) is None:
+            raise ValueError(f"{path}: the parent of joint node {joint_nodes[j]} is not a rotation times a positive uniform "
+                             "scale at the default pose")
+    children = [[] for _ in range(J)]
+    for j in range(J):
+        if parent[j] >= 0:
+            children[parent[j]].append(j)
+    order, stack = [], [j for j in range(J - 1, -1, -1) if parent[j] < 0]
+    while stack:
+        j = stack.pop()
+        order.append(j)
+        stack.extend(reversed(children[j]))
+    if "inverseBindMatrices" in skin:
+        ibm = reader.float_accessor(skin["inverseBindMatrices"])
+        if ibm.shape != (J, 16):
+            raise ValueError(f"{path}: inverseBindMatrices has shape {ibm.shape}, expected ({J}, 16)")
+        ibm = ibm.reshape(J, 4, 4).transpose(0, 2, 1)
+    else:
+        ibm = np.tile(np.eye(4), (J, 1, 1))
+
+    binds, bind_joint, rigid = list(ibm), list(range(J)), {}
+    points, slot_bind, slot_weight = [], [], []
+    for p in included:
+        node, nv = nodes[p.node], len(p.vertices)
+        sb, sw = np.zeros((nv, MAX_INFLUENCES), np.int32), np.zeros((nv, MAX_INFLUENCES))
+        attrs = p.prim["attributes"]
+        if "skin" in node:
+            if p.prim.get("targets") and np.any(np.asarray(node.get("weights", gltf["meshes"][p.mesh].get("weights", []))) != 0):
+                raise ValueError(f"{path}: skinned mesh {p.mesh} has morph targets with non-zero default weights")
+            if any(k.startswith(("JOINTS_", "WEIGHTS_")) and k not in ("JOINTS_0", "JOINTS_1", "WEIGHTS_0", "WEIGHTS_1")
+                   for k in attrs):
+                raise ValueError(f"{path}: mesh {p.mesh} has more than {MAX_INFLUENCES} influences per vertex")
+            sets = [s for s in ("0", "1") if "JOINTS_" + s in attrs or "WEIGHTS_" + s in attrs]
+            if "0" not in sets or any("JOINTS_" + s not in attrs or "WEIGHTS_" + s not in attrs for s in sets):
+                raise ValueError(f"{path}: skinned mesh {p.mesh} lacks a JOINTS_n / WEIGHTS_n pair")
+            jnt = np.concatenate([reader.accessor(attrs["JOINTS_" + s]) for s in sets], 1)
+            wgt = np.concatenate([reader.float_accessor(attrs["WEIGHTS_" + s]) for s in sets], 1)
+            if jnt.dtype.kind != "u" or jnt.dtype.itemsize > 2 or jnt.shape != (nv, 4 * len(sets)) or wgt.shape != jnt.shape:
+                raise ValueError(f"{path}: mesh {p.mesh}'s JOINTS_n / WEIGHTS_n are not u8/u16 and float/normalized VEC4s "
+                                 f"over its {nv} vertices")
+            total = wgt.sum(1, keepdims=True)
+            if not (total > 0).all():
+                raise ValueError(f"{path}: mesh {p.mesh} has a vertex whose weights sum to 0")
+            wgt = wgt / total
+            used = wgt > 0
+            if (jnt[used] >= J).any():
+                raise ValueError(f"{path}: mesh {p.mesh} has a joint index outside the skin's {J} joints")
+            rank = np.argsort(~used, axis=1, kind="stable")       # used slots first, each group in slot order
+            k = used.sum(1, keepdims=True)
+            live = np.arange(jnt.shape[1])[None] < k
+            sb[:, :jnt.shape[1]] = np.where(live, np.take_along_axis(jnt, rank, 1), 0)
+            sw[:, :jnt.shape[1]] = np.where(live, np.take_along_axis(wgt, rank, 1), 0.0)
+            points.append(p.positions)
+        else:
+            k = index[p.node] if p.node in index else joint_ancestor(p.node)[0]
+            if k >= 0:
+                if p.node not in rigid:
+                    rigid[p.node] = len(binds)
+                    binds.append(np.linalg.inv(world0[k]) @ p.world)
+                    bind_joint.append(k)
+                sb[:, 0], sw[:, 0] = rigid[p.node], 1.0
+                points.append(p.positions)
+            else:
+                points.append(p.vertices)
+        slot_bind.append(sb)
+        slot_weight.append(sw)
+    rest = np.concatenate([p.vertices for p in included])
+    rig = GltfRig(joint_nodes=joint_nodes, parent=parent, order=np.array(order, np.int64), translation=translation,
+                  rotation=rotation, scale=scale, from_matrix=np.array(["matrix" in nodes[n] for n in joint_nodes]),
+                  above=above, inverse_bind=ibm, rest=rest, points=np.concatenate(points), binds=np.stack(binds),
+                  bind_joint=np.array(bind_joint, np.int64), slot_bind=np.concatenate(slot_bind),
+                  slot_weight=np.concatenate(slot_weight))
+    posed = rig_pose(rig, world0)
+    diag = float(np.linalg.norm(rest.max(0) - rest.min(0)))
+    err = float(np.abs(posed - rest).max()) if len(rest) else 0.0
+    if err > BIND_TOLERANCE * max(diag, np.finfo(float).tiny):
+        raise ValueError(f"{path}: the default pose is not the bind pose: it moves a vertex by {err:.3e}, more than "
+                         f"{BIND_TOLERANCE:g} of the rest bounding-box diagonal {diag:.3e}")
+    return rig
+
+
+def rig_pose(rig: GltfRig, joint_world: np.ndarray) -> np.ndarray:
+    """(V, 3) vertices of `rig` for the (J, 4, 4) joint world matrices, by plain float64 linear blend skinning (static
+    vertices at rest)."""
+    skin = np.einsum("bij,bjk->bik", joint_world[rig.bind_joint], rig.binds)
+    out = np.zeros_like(rig.rest)
+    for k in range(MAX_INFLUENCES):
+        m = skin[rig.slot_bind[:, k]]
+        out += rig.slot_weight[:, k:k + 1] * (np.einsum("vij,vj->vi", m[:, :3, :3], rig.points) + m[:, :3, 3])
+    static = ~(rig.slot_weight[:, 0] > 0)
+    out[static] = rig.rest[static]
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------------------ writing
@@ -710,6 +973,69 @@ def write_skinned_glb(path, fit, faces, fps: float = 8, visual=None) -> None:
             channels.append({"sampler": len(samplers) - 1, "target": {"node": joint_nodes[j], "path": path_}})
     gltf["animations"] = [{"name": "Animation", "channels": channels, "samplers": samplers}]
     b.write(path, gltf)
+
+
+def write_rig_animation(src_path, out_path, rig: GltfRig, fit, fps: float = 8) -> None:
+    """Write the GLB at `src_path` to `out_path` with a `rig.RigFit` of its `load_rig` rig as a new first animation.
+
+    The JSON and BIN are kept except for: joints stored as `matrix` become their TRS (glTF does not animate `matrix`
+    nodes); a LINEAR animation "ActionMesh" inserted as animations[0], with keys at k / fps, a float32 rotation channel
+    for every joint (each key's sign chosen so that its dot product with the previous key is >= 0) and a translation
+    channel for each root joint; its accessors and bufferViews appended, their data at the end of the BIN chunk (4-byte
+    aligned) and buffers[0].byteLength updated.  The file stays in its own frame."""
+    gltf, binary = _parse_glb(Path(src_path).read_bytes(), src_path)
+    gltf = copy.deepcopy(gltf)
+    buffers = gltf.get("buffers") or []
+    if binary is None or not buffers or "uri" in buffers[0]:
+        raise ValueError(f"{src_path}: the rig animation is written into a GLB whose buffer 0 is its BIN chunk")
+    skins_joints = [s["joints"] for s in gltf.get("skins", [])]
+    if list(rig.joint_nodes) not in skins_joints:
+        raise ValueError(f"{src_path}: the rig's joints are not a skin of this file")
+    quat = np.array(fit.rotations, dtype=np.float64)
+    trans = np.asarray(fit.translations, dtype=np.float64)
+    T, J = quat.shape[:2]
+    if J != len(rig.joint_nodes) or quat.shape != (T, J, 4) or trans.shape != (T, J, 3) or T < 1:
+        raise ValueError(f"the fit's rotations {quat.shape} and translations {trans.shape} do not match the rig's {len(rig.joint_nodes)} joints")
+    for k in range(1, T):
+        quat[k] *= np.where((quat[k] * quat[k - 1]).sum(-1) < 0, -1.0, 1.0)[:, None]
+    nodes = gltf["nodes"]
+    for j, n in enumerate(rig.joint_nodes):
+        if "matrix" in nodes[n]:
+            del nodes[n]["matrix"]
+            nodes[n]["translation"] = rig.translation[j].tolist()
+            nodes[n]["rotation"] = rig.rotation[j].tolist()
+            nodes[n]["scale"] = rig.scale[j].tolist()
+    out = bytearray(binary)
+    out += b"\0" * ((-len(out)) % 4)
+    views, accessors = gltf.setdefault("bufferViews", []), gltf.setdefault("accessors", [])
+
+    def accessor(arr: np.ndarray, type_: str, min_max: bool = False) -> int:
+        arr = np.ascontiguousarray(arr, dtype=np.float32)
+        out.extend(b"\0" * ((-len(out)) % 4))
+        views.append({"buffer": 0, "byteOffset": len(out), "byteLength": arr.nbytes})
+        out.extend(arr.tobytes())
+        acc = {"bufferView": len(views) - 1, "componentType": F32, "count": int(arr.shape[0]), "type": type_}
+        if min_max:
+            acc["min"], acc["max"] = arr.min(0).tolist(), arr.max(0).tolist()
+        accessors.append(acc)
+        return len(accessors) - 1
+
+    times = accessor((np.arange(T, dtype=np.float64) / fps).reshape(-1, 1), "SCALAR", min_max=True)
+    samplers, channels = [], []
+    for j, n in enumerate(rig.joint_nodes):
+        for path_, data, type_, on in (("rotation", quat[:, j], "VEC4", True),
+                                       ("translation", trans[:, j], "VEC3", rig.parent[j] < 0)):
+            if on:
+                samplers.append({"input": times, "output": accessor(data, type_), "interpolation": "LINEAR"})
+                channels.append({"sampler": len(samplers) - 1, "target": {"node": int(n), "path": path_}})
+    gltf["animations"] = [{"name": "ActionMesh", "channels": channels, "samplers": samplers}] + gltf.get("animations", [])
+    out += b"\0" * ((-len(out)) % 4)
+    buffers[0]["byteLength"] = len(out)
+    js = json.dumps(gltf, separators=(",", ":")).encode("utf-8")
+    js += b" " * ((-len(js)) % 4)
+    chunks = struct.pack("<II", len(js), CHUNK_JSON) + js + struct.pack("<II", len(out), CHUNK_BIN) + bytes(out)
+    with open(out_path, "wb") as f:
+        f.write(GLB_MAGIC + struct.pack("<II", 2, 12 + len(chunks)) + chunks)
 
 
 # ------------------------------------------------------------------------------------------------------- the reference's IO

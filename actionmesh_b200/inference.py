@@ -1,14 +1,15 @@
 """The command line: video (+ optional .glb mesh) -> animated meshes on disk, on this package alone.
 
     python -m actionmesh_b200.inference --input clip.mp4 [--mesh_input mesh.glb] [--output_dir DIR] [--fast] [--low_ram]
-                                        [--render_texture] [--skinning_bones N]
+                                        [--render_texture] [--skinning_bones N] [--keep_rig]
 
 One entry point for the reference's `inference/video_to_animated_mesh.py` and `inference/video_and_3d_to_animated_mesh.py`
 (`--mesh_input` selects the second), with their flags and defaults plus `--weights_root`.  It writes, in `--output_dir`
 (default outputs/<input stem>): mesh_00.glb ..., deformations_vertices.npy, deformations_faces.npy, animated_mesh.glb and
 grid_normal.mp4, and with `--render_texture` also grid_texture.mp4 (the meshes shaded with the input mesh's texture, or
 with the default colour), and with `--skinning_bones N` also skinned_mesh.glb (the same animation as N bones and skin
-weights fitted on the GPU, `skinning.fit_skinning`).  `--blender_path` and `--dtype` are accepted so that the reference's documented command lines run
+weights fitted on the GPU, `skinning.fit_skinning`), and with `--keep_rig` (a rigged `--mesh_input`) also rigged_mesh.glb (the
+input file with its own skeleton animated: joint rotations fitted on the GPU, `rig.fit_rig_animation`).  `--blender_path` and `--dtype` are accepted so that the reference's documented command lines run
 unchanged, and have no effect: the animated GLB is written without Blender, and the CUDA path owns its precision.
 """
 from __future__ import annotations
@@ -24,8 +25,10 @@ import numpy as np
 import torch
 
 from . import render
+from . import rig as rig_fit
 from . import skinning
-from .gltf import load_glb, save_deformation, save_meshes, write_animated_glb, write_skinned_glb
+from .gltf import GltfRig, load_glb, load_rig, save_deformation, save_meshes, write_animated_glb, write_rig_animation, \
+    write_skinned_glb
 from .pipeline import ActionMeshB200Pipeline, ActionMeshB200PipelineWithMeshInput
 from .video_input import load_frames
 
@@ -37,11 +40,13 @@ ANIMATION_FPS = 8
 
 @torch.no_grad()
 def run_actionmesh(pipeline, input: str, output_dir: str, seed: int = 44, mesh_input: Optional[str] = None,
-                   render_texture: bool = False, skinning_bones: int = 0, **overrides) -> list:
+                   render_texture: bool = False, skinning_bones: int = 0, rig: Optional[GltfRig] = None,
+                   **overrides) -> list:
     """The reference scripts' `run_actionmesh`: load the frames (and the mesh), run `pipeline`, write every output file
     into `output_dir` -> the meshes.  `render_texture` adds grid_texture.mp4, shaded with the input mesh's visual (the one
     the animated GLB gets).  `skinning_bones` > 0 adds skinned_mesh.glb: that many bones fitted to the animated GLB's
-    vertices, written with its faces and visual.  `overrides` are the pipeline's per-call arguments (stage_0_steps, face_decimation,
+    vertices, written with its faces and visual.  `rig` (`load_rig(mesh_input)`) adds rigged_mesh.glb: the input file with
+    its joint rotations fitted to the same vertices.  `overrides` are the pipeline's per-call arguments (stage_0_steps, face_decimation,
     floaters_threshold, stage_1_steps, guidance_scales, anchor_idx)."""
     frames = load_frames(input, max_frames=MAX_FRAMES)
     visual = None
@@ -66,6 +71,14 @@ def run_actionmesh(pipeline, input: str, output_dir: str, seed: int = 44, mesh_i
         skinned = os.path.join(output_dir, "skinned_mesh.glb")
         write_skinned_glb(skinned, fit, faces, fps=ANIMATION_FPS, visual=visual)
         logger.info(f"Skinned GLB saved to {skinned} ({skinning_bones} bones; RMS error {fit.rms_error:.3e}, max error "
+                    f"{fit.max_error:.3e} of the rest bounding-box diagonal)")
+    if rig is not None:
+        if mesh_input is None:
+            raise ValueError("a rig is kept only for a --mesh_input")
+        fit = rig_fit.fit_rig_animation(rig, vertices, device=pipeline.device)
+        rigged = os.path.join(output_dir, "rigged_mesh.glb")
+        write_rig_animation(mesh_input, rigged, rig, fit, fps=ANIMATION_FPS)
+        logger.info(f"Rigged GLB saved to {rigged} ({len(rig.joint_nodes)} joints; RMS error {fit.rms_error:.3e}, max error "
                     f"{fit.max_error:.3e} of the rest bounding-box diagonal)")
     visualizer = render.B200MeshVisualizer(image_size=256)
     if render_texture:
@@ -100,7 +113,12 @@ def parse_args(argv=None) -> argparse.Namespace:
                    help="Also write grid_texture.mp4: the meshes shaded with the input mesh's texture (or a flat colour).")
     p.add_argument("--skinning_bones", type=int, default=0,
                    help="Also write skinned_mesh.glb with this many bones fitted to the animation (at most 256). Default: 0 (off)")
-    return p.parse_args(argv)
+    p.add_argument("--keep_rig", action="store_true",
+                   help="Also write rigged_mesh.glb: the rigged --mesh_input with its own skeleton animated.")
+    args = p.parse_args(argv)
+    if args.keep_rig and args.mesh_input is None:
+        p.error("--keep_rig needs --mesh_input (a rigged .glb)")
+    return args
 
 
 def main(argv=None) -> list:
@@ -110,6 +128,12 @@ def main(argv=None) -> list:
         logger.info("--blender_path has no effect: animated_mesh.glb is written without Blender")
     if args.dtype != "bfloat16":
         logger.info(f"--dtype {args.dtype} has no effect: the CUDA path owns its precision")
+    rig = None
+    if args.keep_rig:
+        try:
+            rig = load_rig(args.mesh_input)        # before any model loads: a file without a usable rig fails fast
+        except ValueError as exc:
+            raise SystemExit(f"--keep_rig: {exc}") from exc
     config_name = "actionmesh_b200_fast.yaml" if args.fast else "actionmesh_b200.yaml"
     output_dir = args.output_dir or f"outputs/{Path(args.input).stem}"
     cls = ActionMeshB200Pipeline if args.mesh_input is None else ActionMeshB200PipelineWithMeshInput
@@ -117,7 +141,7 @@ def main(argv=None) -> list:
     overrides = {k: getattr(args, k) for k in ("stage_0_steps", "face_decimation", "floaters_threshold",
                                                "stage_1_steps", "guidance_scales", "anchor_idx")}
     return run_actionmesh(pipeline, args.input, output_dir, seed=args.seed, mesh_input=args.mesh_input,
-                          render_texture=args.render_texture, skinning_bones=args.skinning_bones, **overrides)
+                          render_texture=args.render_texture, skinning_bones=args.skinning_bones, rig=rig, **overrides)
 
 
 if __name__ == "__main__":

@@ -1095,6 +1095,104 @@ def skin_error(rest: torch.Tensor, vertices: torch.Tensor, transforms: torch.Ten
     return frame_errors, max_error2
 
 
+# ---- rig animation (csrc/rig.cu; DESIGN.md §21) ---------------------------------------------------------------------------------
+# `rig` is a `rig.RigTensors`: parent (J) int32 in a topological order, scale (J, 3), above (J, 12), above_inv (J, 9),
+# binds (NB, 12), bind_joint (NB) int32, world (T, J, 12) and skin (T, NB, 12) outputs; points and rest (V, 3), slot_bind
+# (V, 8) int32, slot_weight (V, 8), scratch.  State: rotations (T, J, 9), translations (T, J, 3).  Contiguous fp64 unless
+# stated.
+
+def _rig_args(rig, rotations: torch.Tensor, translations: torch.Tensor, dev: int) -> tuple:
+    J, NB = rig.parent.shape[0], rig.bind_joint.shape[0]
+    T = rotations.shape[0]
+    for t, shape, name in ((rig.parent, (J,), "parent"), (rig.scale, (J, 3), "scale"), (rig.above, (J, 12), "above"),
+                           (rig.binds, (NB, 12), "binds"), (rig.bind_joint, (NB,), "bind_joint"),
+                           (rotations, (T, J, 9), "rotations"), (translations, (T, J, 3), "translations"),
+                           (rig.world, (T, J, 12), "world"), (rig.skin, (T, NB, 12), "skin")):
+        _icp_tensor(t, shape, name)
+    return (_ptr(rig.parent, torch.int32, "parent", dev), J, _ptr(rig.scale, torch.float64, "scale", dev),
+            _ptr(rig.above, torch.float64, "above", dev)), \
+        (_ptr(rig.binds, torch.float64, "binds", dev), _ptr(rig.bind_joint, torch.int32, "bind_joint", dev), NB, T,
+         _ptr(rig.world, torch.float64, "world", dev), _ptr(rig.skin, torch.float64, "skin", dev))
+
+
+def _rig_vertex_args(rig, vertices: torch.Tensor, T: int, dev: int) -> tuple:
+    V = rig.points.shape[0]
+    for t, shape, name in ((rig.points, (V, 3), "points"), (vertices, (T, V, 3), "vertices"),
+                           (rig.slot_bind, (V, 8), "slot_bind"), (rig.slot_weight, (V, 8), "slot_weight")):
+        _icp_tensor(t, shape, name)
+    return (_ptr(rig.points, torch.float64, "points", dev), _ptr(vertices, torch.float64, "vertices", dev), V,
+            _ptr(rig.slot_bind, torch.int32, "slot_bind", dev), _ptr(rig.slot_weight, torch.float64, "slot_weight", dev))
+
+
+def rig_scratch(frames: int, n_vertices: int, device) -> torch.Tensor:
+    """The fp64 scratch `rig_rotation_update`, `rig_translation_update` and `rig_error` need for these sizes."""
+    n = C.c_int64()
+    _lib.check(_abi.amb_rig_scratch_doubles(int(frames), int(n_vertices), C.byref(n)), "amb_rig_scratch_doubles")
+    return torch.empty(n.value, dtype=torch.float64, device=device)
+
+
+def rig_forward(rig, rotations: torch.Tensor, translations: torch.Tensor) -> None:
+    """Forward kinematics: rig.world = every joint's world transform and rig.skin = every bind's skinning transform, per
+    frame."""
+    dev = _device(rotations, "rotations")
+    head, tail = _rig_args(rig, rotations, translations, dev)
+    _launch(_abi.amb_rig_forward, 1, *head, _ptr(rotations, torch.float64, "rotations", dev),
+            _ptr(translations, torch.float64, "translations", dev), *tail, tag="rig_forward")
+
+
+def _rig_list(lst: torch.Tensor) -> int:
+    if lst.dim() != 1 or not lst.is_contiguous():
+        raise _lib.AmbError(f"list: expected a contiguous 1-D tensor, got {tuple(lst.shape)}")
+    return lst.shape[0]
+
+
+def rig_rotation_update(rig, rotations: torch.Tensor, translations: torch.Tensor, vertices: torch.Tensor,
+                        lst: torch.Tensor, joint: int, subtree_end: int) -> None:
+    """Refit rotations[:, joint] (in place) to `vertices` (T, V, 3) over the vertices `lst` (int32) that the subtree
+    [joint, subtree_end) influences; nothing runs when `lst` is empty."""
+    dev = _device(rotations, "rotations")
+    head, tail = _rig_args(rig, rotations, translations, dev)
+    n = _rig_list(lst)
+    _launch(_abi.amb_rig_rotation_update, 3 if n else 0, *head, _ptr(rotations, torch.float64, "rotations", dev),
+            _ptr(translations, torch.float64, "translations", dev), *tail,
+            *_rig_vertex_args(rig, vertices, rotations.shape[0], dev), _ptr(lst, torch.int32, "list", dev), n, int(joint),
+            int(subtree_end), _ptr(rig.scratch, torch.float64, "scratch", dev), tag="rig_rotation_update")
+
+
+def rig_translation_update(rig, rotations: torch.Tensor, translations: torch.Tensor, vertices: torch.Tensor,
+                           lst: torch.Tensor, joint: int, subtree_end: int) -> None:
+    """Refit the root joint's translations[:, joint] (in place) to `vertices` over the vertices `lst` its subtree
+    [joint, subtree_end) influences; nothing runs when `lst` is empty."""
+    dev = _device(rotations, "rotations")
+    head, tail = _rig_args(rig, rotations, translations, dev)
+    _icp_tensor(rig.above_inv, (rig.parent.shape[0], 9), "above_inv")
+    n = _rig_list(lst)
+    _launch(_abi.amb_rig_translation_update, 3 if n else 0, *head, _ptr(rig.above_inv, torch.float64, "above_inv", dev),
+            _ptr(rotations, torch.float64, "rotations", dev), _ptr(translations, torch.float64, "translations", dev), *tail,
+            *_rig_vertex_args(rig, vertices, rotations.shape[0], dev), _ptr(lst, torch.int32, "list", dev), n, int(joint),
+            int(subtree_end), _ptr(rig.scratch, torch.float64, "scratch", dev), tag="rig_translation_update")
+
+
+def rig_error(rig, rotations: torch.Tensor, translations: torch.Tensor, vertices: torch.Tensor,
+              frame_errors: Optional[torch.Tensor] = None) -> tuple[torch.Tensor, torch.Tensor]:
+    """Reconstruction error of the rig's animation -> (frame_errors (T + 1) fp64 = sum |v^ - v|^2 per frame then their
+    sum, written into `frame_errors` when given; max_error2 (1) fp64 = the largest |v^ - v|^2)."""
+    dev = _device(rotations, "rotations")
+    head, tail = _rig_args(rig, rotations, translations, dev)
+    T = rotations.shape[0]
+    _icp_tensor(rig.rest, tuple(rig.points.shape), "rest")
+    if frame_errors is None:
+        frame_errors = torch.empty(T + 1, dtype=torch.float64, device=rotations.device)
+    _icp_tensor(frame_errors, (T + 1,), "frame_errors")
+    max_error2 = torch.empty(1, dtype=torch.float64, device=rotations.device)
+    _launch(_abi.amb_rig_error, 3, *head, _ptr(rotations, torch.float64, "rotations", dev),
+            _ptr(translations, torch.float64, "translations", dev), *tail, _ptr(rig.rest, torch.float64, "rest", dev),
+            *_rig_vertex_args(rig, vertices, T, dev), _ptr(rig.scratch, torch.float64, "scratch", dev),
+            _ptr(frame_errors, torch.float64, "frame_errors", dev), _ptr(max_error2, torch.float64, "max_error2", dev),
+            tag="rig_error")
+    return frame_errors, max_error2
+
+
 # ---- background removal: RMBG-1.4's resampling, im2col, mask head and refinement (csrc/rmbg.cu) ------------------------------
 # Activations are fp32 NHWC feature maps held as 2-D (H * W, pixel stride) tensors with unit channel stride: a GEMM output
 # padded to 64 columns is read in place, its first C columns being the channels.

@@ -487,6 +487,46 @@ int amb_skin_error(const double* rest, const double* vertices, int frames, int64
                    int n_bones, const int32_t* joints, const double* weights, double* scratch, double* frame_errors,
                    double* max_error2, amb_stream_t stream);
 
+/* ---- rig animation: joint rotations of an existing skeleton fitted to a vertex animation (csrc/rig.cu; DESIGN.md §21) -------
+ * actionmesh_b200/rig.py drives the calls.  All arithmetic is fp64 with each operation rounded on its own, in the order
+ * DESIGN.md §21 states; no result depends on scheduling.  Transforms are 12 doubles (L row-major, then t: p -> L p + t).
+ * The rig: J joints in a topological order (parent (J) int32, parent[j] < j, -1 for a root; not checked on the device),
+ * scale (J, 3), above (J, 12) = the fixed transform above each root joint, binds (NB, 12) bind matrices acting on `points`,
+ * bind_joint (NB) int32 in [0, J).  The state: rotations (T, J, 9) local R, translations (T, J, 3) local translations.
+ * world (T, J, 12) and skin (T, NB, 12) receive G_j = P_j [R_j diag(s_j) | tau_j] (P_j = G_parent or above[j]) and
+ * K_b = G_{bind_joint[b]} B_b.  Vertices: points, rest (V, 3) and vertices (T, V, 3) fp64; slot_bind (V, 8) int32 and
+ * slot_weight (V, 8) fp64, used slots (weight > 0) first, a vertex with slot 0 unused showing rest.  1 <= J <= 1024,
+ * 1 <= NB <= 2^20, 1 <= T <= 65535, 1 <= V < 2^31 - 256.  list (n_list) int32: the vertices whose used slots hold a joint of
+ * the subtree [joint, subtree_end).
+ *  rig_scratch_doubles: the fp64 scratch the updates and rig_error need for T frames and V vertices.
+ *  rig_forward: world and skin from the state.
+ *  rig_rotation_update: forward, then rotations[:, joint] = the rotation minimising the squared error with everything else
+ *    fixed (Horn's method on the subtree's moments).  No launch when n_list == 0.
+ *  rig_translation_update: forward, then translations[:, joint] += above_inv[joint] (sum m (v - v^)) / sum m^2 for a root
+ *    joint (above_inv (J, 9) row-major), m the subtree's weight of each listed vertex.  No launch when n_list == 0.
+ *  rig_error: forward, then frame_errors (T + 1) = sum_i |v^_i - v_i|^2 per frame, then their sum; max_error2 (1) = the
+ *    largest |v^_i - v_i|^2. */
+int amb_rig_scratch_doubles(int frames, int64_t n_vertices, int64_t* out_doubles);
+int amb_rig_forward(const int32_t* parent, int n_joints, const double* scale, const double* above, const double* rotations,
+                    const double* translations, const double* binds, const int32_t* bind_joint, int n_binds, int frames,
+                    double* world, double* skin, amb_stream_t stream);
+int amb_rig_rotation_update(const int32_t* parent, int n_joints, const double* scale, const double* above, double* rotations,
+                            const double* translations, const double* binds, const int32_t* bind_joint, int n_binds,
+                            int frames, double* world, double* skin, const double* points, const double* vertices,
+                            int64_t n_vertices, const int32_t* slot_bind, const double* slot_weight, const int32_t* list,
+                            int64_t n_list, int joint, int subtree_end, double* scratch, amb_stream_t stream);
+int amb_rig_translation_update(const int32_t* parent, int n_joints, const double* scale, const double* above,
+                               const double* above_inv, const double* rotations, double* translations, const double* binds,
+                               const int32_t* bind_joint, int n_binds, int frames, double* world, double* skin,
+                               const double* points, const double* vertices, int64_t n_vertices, const int32_t* slot_bind,
+                               const double* slot_weight, const int32_t* list, int64_t n_list, int joint, int subtree_end,
+                               double* scratch, amb_stream_t stream);
+int amb_rig_error(const int32_t* parent, int n_joints, const double* scale, const double* above, const double* rotations,
+                  const double* translations, const double* binds, const int32_t* bind_joint, int n_binds, int frames,
+                  double* world, double* skin, const double* rest, const double* points, const double* vertices,
+                  int64_t n_vertices, const int32_t* slot_bind, const double* slot_weight, double* scratch,
+                  double* frame_errors, double* max_error2, amb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
