@@ -908,6 +908,53 @@ def _quaternions(rot: np.ndarray) -> np.ndarray:
     return q / np.linalg.norm(q, axis=-1, keepdims=True)
 
 
+def _checked_skin(rest: np.ndarray, faces, joints, weights, n_joints: int, what: str,
+                  noun: str) -> tuple[np.ndarray, np.ndarray]:
+    """(faces (F, 3), weights divided by their row sums) after the checks every skinned file makes; `what` names the
+    file and `noun` its joints in the messages."""
+    f = np.asarray(faces).reshape(-1, 3)
+    if not len(f):
+        raise ValueError(f"{what} needs at least one face")
+    _check_faces(f, len(rest))
+    j = np.asarray(joints)
+    if n_joints > 256 or j.shape != (len(rest), 4) or j.min() < 0 or j.max() >= n_joints:
+        raise ValueError(f"joints must be (V, 4) indices of the {n_joints} {noun} (at most 256)")
+    w = np.asarray(weights, dtype=np.float64)
+    total = w.sum(1, keepdims=True) if w.ndim == 2 else np.zeros(1)
+    if w.shape != (len(rest), 4) or (w < 0).any() or not (total > 0).all():
+        raise ValueError("weights must be (V, 4), non-negative, with a positive sum per vertex")
+    return f, w / total
+
+
+def _key_quaternions(rot: np.ndarray) -> np.ndarray:
+    """(T, J, 3, 3) rotations -> (T, J, 4) quaternions of M R M^T (M = ANIMATED_GLB_MAP), each key's sign chosen so that its
+    dot product with the previous key's is >= 0."""
+    quat = _quaternions(ANIMATED_GLB_MAP @ rot @ ANIMATED_GLB_MAP.T)
+    for k in range(1, len(quat)):
+        quat[k] *= np.where((quat[k] * quat[k - 1]).sum(-1) < 0, -1.0, 1.0)[:, None]
+    return quat
+
+
+def _skinned_mesh(b: _GlbBuilder, gltf: dict, rest: np.ndarray, joints, weights: np.ndarray, f: np.ndarray, visual) -> None:
+    """gltf["meshes"] = one "SkinnedMesh": POSITION = M p (float32 with min/max), JOINTS_0 (u8), WEIGHTS_0 (float32,
+    rows already normalised), with the visual's UVs and material (the default blue without one), or one primitive per
+    range of a `GltfMultiVisual`."""
+    per_vertex = [("POSITION", (rest @ ANIMATED_GLB_MAP.T).astype(np.float32), F32, "VEC3", True),
+                  ("JOINTS_0", np.asarray(joints, dtype=np.uint8), U8, "VEC4", False),
+                  ("WEIGHTS_0", weights.astype(np.float32), F32, "VEC4", False)]
+    if isinstance(visual, GltfMultiVisual):
+        check_multi_visual(visual, len(rest), f)
+        gltf["meshes"] = [{"name": "SkinnedMesh", "primitives": b.add_primitives(gltf, visual, f, per_vertex)}]
+    else:
+        attributes = {name: b.accessor(arr, comp, type_, ARRAY_BUFFER, min_max=mm) for name, arr, comp, type_, mm in per_vertex}
+        indices = b.accessor(f.reshape(-1, 1), U32, "SCALAR", ELEMENT_ARRAY_BUFFER)
+        b.add_visual(gltf, attributes, visual, len(rest))
+        if "materials" not in gltf:
+            gltf["materials"] = [copy.deepcopy(DEFAULT_MATERIAL)]
+        gltf["meshes"] = [{"name": "SkinnedMesh", "primitives": [{"attributes": attributes, "indices": indices,
+                                                                  "material": 0, "mode": TRIANGLES}]}]
+
+
 def write_skinned_glb(path, fit, faces, fps: float = 8, visual=None) -> None:
     """Write a `skinning.SkinningFit` on (F, 3) `faces` as a skinned GLB: one rest mesh, n_bones joints and one LINEAR
     animation, in the coordinates of `write_animated_glb` (DESIGN §20).
@@ -921,18 +968,9 @@ def write_skinned_glb(path, fit, faces, fps: float = 8, visual=None) -> None:
     primitive per range, each with JOINTS_0 and WEIGHTS_0 over its range under the one skin and its own material (the
     default blue when it has none)."""
     rest = np.asarray(fit.rest, dtype=np.float64)
-    f = np.asarray(faces).reshape(-1, 3)
     rot, trans, centres = (np.asarray(a, dtype=np.float64) for a in (fit.rotations, fit.translations, fit.centres))
     T, B = rot.shape[:2]
-    if not len(f):
-        raise ValueError("a skinned GLB needs at least one face")
-    _check_faces(f, len(rest))
-    if B > 256 or fit.joints.shape != (len(rest), 4) or np.asarray(fit.joints).min() < 0 or np.asarray(fit.joints).max() >= B:
-        raise ValueError(f"joints must be (V, 4) indices of the {B} bones (at most 256)")
-    w = np.asarray(fit.weights, dtype=np.float64)
-    total = w.sum(1, keepdims=True)
-    if w.shape != (len(rest), 4) or (w < 0).any() or not (total > 0).all():
-        raise ValueError("weights must be (V, 4), non-negative, with a positive sum per vertex")
+    f, w = _checked_skin(rest, faces, fit.joints, fit.weights, B, "a skinned GLB", "bones")
     M = ANIMATED_GLB_MAP
     mc = centres @ M.T
     joint_nodes = list(range(2, 2 + B))
@@ -940,28 +978,13 @@ def write_skinned_glb(path, fit, faces, fps: float = 8, visual=None) -> None:
                   "nodes": [{"mesh": 0, "skin": 0, "name": "SkinnedMesh"}, {"name": "Armature", "children": joint_nodes}]
                   + [{"name": f"Bone_{j}", "translation": mc[j].tolist()} for j in range(B)]}
     b = _GlbBuilder()
-    per_vertex = [("POSITION", (rest @ M.T).astype(np.float32), F32, "VEC3", True),
-                  ("JOINTS_0", np.asarray(fit.joints, dtype=np.uint8), U8, "VEC4", False),
-                  ("WEIGHTS_0", (w / total).astype(np.float32), F32, "VEC4", False)]
-    if isinstance(visual, GltfMultiVisual):
-        check_multi_visual(visual, len(rest), f)
-        gltf["meshes"] = [{"name": "SkinnedMesh", "primitives": b.add_primitives(gltf, visual, f, per_vertex)}]
-    else:
-        attributes = {name: b.accessor(arr, comp, type_, ARRAY_BUFFER, min_max=mm) for name, arr, comp, type_, mm in per_vertex}
-        indices = b.accessor(f.reshape(-1, 1), U32, "SCALAR", ELEMENT_ARRAY_BUFFER)
-        b.add_visual(gltf, attributes, visual, len(rest))
-        if "materials" not in gltf:
-            gltf["materials"] = [copy.deepcopy(DEFAULT_MATERIAL)]
-        gltf["meshes"] = [{"name": "SkinnedMesh", "primitives": [{"attributes": attributes, "indices": indices,
-                                                                  "material": 0, "mode": TRIANGLES}]}]
+    _skinned_mesh(b, gltf, rest, fit.joints, w, f, visual)
     ibm = np.tile(np.eye(4), (B, 1, 1))
     ibm[:, :3, 3] = -mc
     gltf["skins"] = [{"joints": joint_nodes, "skeleton": 1,
                       "inverseBindMatrices": b.accessor(ibm.transpose(0, 2, 1).reshape(B, 16).astype(np.float32), F32,
                                                         "MAT4")}]
-    quat = _quaternions(M @ rot @ M.T)                                                   # (T, B, 4)
-    for k in range(1, T):
-        quat[k] *= np.where((quat[k] * quat[k - 1]).sum(-1) < 0, -1.0, 1.0)[:, None]
+    quat = _key_quaternions(rot)                                                         # (T, B, 4)
     node_t = (np.einsum("tbij,bj->tbi", rot, centres) + trans) @ M.T                    # (T, B, 3)
     times = b.accessor((np.arange(T, dtype=np.float64) / fps).astype(np.float32).reshape(-1, 1), F32, "SCALAR",
                        min_max=True)
@@ -971,6 +994,54 @@ def write_skinned_glb(path, fit, faces, fps: float = 8, visual=None) -> None:
             samplers.append({"input": times, "output": b.accessor(data.astype(np.float32), F32, type_),
                              "interpolation": "LINEAR"})
             channels.append({"sampler": len(samplers) - 1, "target": {"node": joint_nodes[j], "path": path_}})
+    gltf["animations"] = [{"name": "Animation", "channels": channels, "samplers": samplers}]
+    b.write(path, gltf)
+
+
+def write_auto_rig_glb(path, fit, faces, fps: float = 8, visual=None) -> None:
+    """Write an `autorig.AutoRigFit` on (F, 3) `faces` as a rigged GLB in the coordinates of `write_animated_glb`
+    (DESIGN §22): the mesh and material as `write_skinned_glb` writes them, and a joint hierarchy "Joint_<k>" nested under
+    "Armature" in the fit's depth-first order.
+
+    Joint k's node translation is M (c_k - c_parent) (M c_root for the root), its inverse bind translate(-M c_k).  One
+    LINEAR animation keys, at k / fps, every joint's rotation (the quaternion of M R M^T, each key's sign chosen closest
+    to the previous key's) and the root's translation M tau.  Conjugating by the reflection M keeps every composition, so
+    key k shows M v^ of the fit's frame k."""
+    rest = np.asarray(fit.rest, dtype=np.float64)
+    rot = np.asarray(fit.rotation_matrices, dtype=np.float64)
+    T, J = rot.shape[:2]
+    parent = np.asarray(fit.parent, np.int64)
+    f, w = _checked_skin(rest, faces, fit.joints, fit.weights, J, "a rigged GLB", "joints")
+    if parent.shape != (J,) or parent[0] != -1 or (parent[1:] < 0).any() or (parent[1:] >= np.arange(1, J)).any():
+        raise ValueError("parent must list a depth-first tree rooted at joint 0")
+    M = ANIMATED_GLB_MAP
+    mc = np.asarray(fit.positions, dtype=np.float64) @ M.T
+    joint_nodes = list(range(2, 2 + J))
+    nodes = [{"mesh": 0, "skin": 0, "name": "RiggedMesh"}, {"name": "Armature", "children": [2]}]
+    for k in range(J):
+        node = {"name": f"Joint_{k}", "translation": (mc[k] - mc[parent[k]] if k else mc[k]).tolist()}
+        children = [2 + c for c in np.flatnonzero(parent == k)]
+        if children:
+            node["children"] = [int(c) for c in children]
+        nodes.append(node)
+    gltf: dict = {"scene": 0, "scenes": [{"nodes": [0, 1]}], "nodes": nodes}
+    b = _GlbBuilder()
+    _skinned_mesh(b, gltf, rest, fit.joints, w, f, visual)
+    ibm = np.tile(np.eye(4), (J, 1, 1))
+    ibm[:, :3, 3] = -mc
+    gltf["skins"] = [{"joints": joint_nodes, "skeleton": 1,
+                      "inverseBindMatrices": b.accessor(ibm.transpose(0, 2, 1).reshape(J, 16).astype(np.float32), F32,
+                                                        "MAT4")}]
+    quat = _key_quaternions(rot)                                                         # (T, J, 4)
+    times = b.accessor((np.arange(T, dtype=np.float64) / fps).astype(np.float32).reshape(-1, 1), F32, "SCALAR",
+                       min_max=True)
+    samplers = [{"input": times, "output": b.accessor((np.asarray(fit.root_translations) @ M.T).astype(np.float32), F32,
+                                                      "VEC3"), "interpolation": "LINEAR"}]
+    channels = [{"sampler": 0, "target": {"node": joint_nodes[0], "path": "translation"}}]
+    for k in range(J):
+        samplers.append({"input": times, "output": b.accessor(quat[:, k].astype(np.float32), F32, "VEC4"),
+                         "interpolation": "LINEAR"})
+        channels.append({"sampler": len(samplers) - 1, "target": {"node": joint_nodes[k], "path": "rotation"}})
     gltf["animations"] = [{"name": "Animation", "channels": channels, "samplers": samplers}]
     b.write(path, gltf)
 

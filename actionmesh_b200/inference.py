@@ -1,7 +1,7 @@
 """The command line: video (+ optional .glb mesh) -> animated meshes on disk, on this package alone.
 
     python -m actionmesh_b200.inference --input clip.mp4 [--mesh_input mesh.glb] [--output_dir DIR] [--fast] [--low_ram]
-                                        [--render_texture] [--skinning_bones N] [--keep_rig]
+                                        [--render_texture] [--skinning_bones N] [--keep_rig] [--auto_rig N]
 
 One entry point for the reference's `inference/video_to_animated_mesh.py` and `inference/video_and_3d_to_animated_mesh.py`
 (`--mesh_input` selects the second), with their flags and defaults plus `--weights_root`.  It writes, in `--output_dir`
@@ -9,7 +9,9 @@ One entry point for the reference's `inference/video_to_animated_mesh.py` and `i
 grid_normal.mp4, and with `--render_texture` also grid_texture.mp4 (the meshes shaded with the input mesh's texture, or
 with the default colour), and with `--skinning_bones N` also skinned_mesh.glb (the same animation as N bones and skin
 weights fitted on the GPU, `skinning.fit_skinning`), and with `--keep_rig` (a rigged `--mesh_input`) also rigged_mesh.glb (the
-input file with its own skeleton animated: joint rotations fitted on the GPU, `rig.fit_rig_animation`).  `--blender_path` and `--dtype` are accepted so that the reference's documented command lines run
+input file with its own skeleton animated: joint rotations fitted on the GPU, `rig.fit_rig_animation`), and with
+`--auto_rig N` also auto_rigged_mesh.glb (a skeleton of N joints found from the animation itself, its joint rotations
+and skin weights fitted on the GPU, `autorig.fit_auto_rig`).  `--blender_path` and `--dtype` are accepted so that the reference's documented command lines run
 unchanged, and have no effect: the animated GLB is written without Blender, and the CUDA path owns its precision.
 """
 from __future__ import annotations
@@ -24,11 +26,11 @@ from typing import Optional
 import numpy as np
 import torch
 
-from . import render
+from . import autorig, render
 from . import rig as rig_fit
 from . import skinning
 from .gltf import GltfRig, load_glb, load_rig, save_deformation, save_meshes, write_animated_glb, write_rig_animation, \
-    write_skinned_glb
+    write_auto_rig_glb, write_skinned_glb
 from .pipeline import ActionMeshB200Pipeline, ActionMeshB200PipelineWithMeshInput
 from .video_input import load_frames
 
@@ -41,12 +43,13 @@ ANIMATION_FPS = 8
 @torch.no_grad()
 def run_actionmesh(pipeline, input: str, output_dir: str, seed: int = 44, mesh_input: Optional[str] = None,
                    render_texture: bool = False, skinning_bones: int = 0, rig: Optional[GltfRig] = None,
-                   **overrides) -> list:
+                   auto_rig_joints: int = 0, **overrides) -> list:
     """The reference scripts' `run_actionmesh`: load the frames (and the mesh), run `pipeline`, write every output file
     into `output_dir` -> the meshes.  `render_texture` adds grid_texture.mp4, shaded with the input mesh's visual (the one
     the animated GLB gets).  `skinning_bones` > 0 adds skinned_mesh.glb: that many bones fitted to the animated GLB's
     vertices, written with its faces and visual.  `rig` (`load_rig(mesh_input)`) adds rigged_mesh.glb: the input file with
-    its joint rotations fitted to the same vertices.  `overrides` are the pipeline's per-call arguments (stage_0_steps, face_decimation,
+    its joint rotations fitted to the same vertices.  `auto_rig_joints` > 0 adds auto_rigged_mesh.glb: a skeleton of that
+    many joints found from the same vertices and faces, written with the visual.  `overrides` are the pipeline's per-call arguments (stage_0_steps, face_decimation,
     floaters_threshold, stage_1_steps, guidance_scales, anchor_idx)."""
     frames = load_frames(input, max_frames=MAX_FRAMES)
     visual = None
@@ -80,6 +83,13 @@ def run_actionmesh(pipeline, input: str, output_dir: str, seed: int = 44, mesh_i
         write_rig_animation(mesh_input, rigged, rig, fit, fps=ANIMATION_FPS)
         logger.info(f"Rigged GLB saved to {rigged} ({len(rig.joint_nodes)} joints; RMS error {fit.rms_error:.3e}, max error "
                     f"{fit.max_error:.3e} of the rest bounding-box diagonal)")
+    if auto_rig_joints > 0:
+        fit = autorig.fit_auto_rig(vertices, faces, auto_rig_joints, device=pipeline.device)
+        auto_rigged = os.path.join(output_dir, "auto_rigged_mesh.glb")
+        write_auto_rig_glb(auto_rigged, fit, faces, fps=ANIMATION_FPS, visual=visual)
+        logger.info(f"Auto-rigged GLB saved to {auto_rigged} ({auto_rig_joints} joints; RMS error {fit.rms_error:.3e} against "
+                    f"{fit.ssdr_rms_error:.3e} for flat bones, max error {fit.max_error:.3e} of the rest bounding-box "
+                    f"diagonal)")
     visualizer = render.B200MeshVisualizer(image_size=256)
     if render_texture:
         visualizer.render(meshes, pipeline.device, output_dir, frames.frames, modalities=("normal", "texture"),
@@ -115,7 +125,12 @@ def parse_args(argv=None) -> argparse.Namespace:
                    help="Also write skinned_mesh.glb with this many bones fitted to the animation (at most 256). Default: 0 (off)")
     p.add_argument("--keep_rig", action="store_true",
                    help="Also write rigged_mesh.glb: the rigged --mesh_input with its own skeleton animated.")
+    p.add_argument("--auto_rig", type=int, default=0, metavar="N",
+                   help="Also write auto_rigged_mesh.glb: a skeleton of N joints found from the animation, its joint "
+                        "rotations and skin weights fitted to it (at most 256). Default: 0 (off)")
     args = p.parse_args(argv)
+    if not 0 <= args.auto_rig <= 256:
+        p.error(f"--auto_rig must be in [0, 256], got {args.auto_rig}")
     if args.keep_rig and args.mesh_input is None:
         p.error("--keep_rig needs --mesh_input (a rigged .glb)")
     return args
@@ -141,7 +156,8 @@ def main(argv=None) -> list:
     overrides = {k: getattr(args, k) for k in ("stage_0_steps", "face_decimation", "floaters_threshold",
                                                "stage_1_steps", "guidance_scales", "anchor_idx")}
     return run_actionmesh(pipeline, args.input, output_dir, seed=args.seed, mesh_input=args.mesh_input,
-                          render_texture=args.render_texture, skinning_bones=args.skinning_bones, rig=rig, **overrides)
+                          render_texture=args.render_texture, skinning_bones=args.skinning_bones, rig=rig,
+                          auto_rig_joints=args.auto_rig, **overrides)
 
 
 if __name__ == "__main__":

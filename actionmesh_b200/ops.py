@@ -1193,6 +1193,110 @@ def rig_error(rig, rotations: torch.Tensor, translations: torch.Tensor, vertices
     return frame_errors, max_error2
 
 
+# ---- automatic rig (csrc/autorig.cu; DESIGN.md §22) ----------------------------------------------------------------------------
+# Bones i < j of B form pair p = i (2B - i - 1) / 2 + (j - i - 1), P = B (B - 1) / 2 pairs.  joints (V, 4) int32, weights
+# (V, 4) fp64, a slot being used when its weight is > 0.
+
+def autorig_pair_stats(rest: torch.Tensor, faces: torch.Tensor, joints: torch.Tensor, weights: torch.Tensor,
+                       n_bones: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """Every face edge whose ends have different dominant bones counts for its pair -> (pair_count (P) int32, pair_prior
+    (P, 3) fp64 = the mean of those edges' rest midpoints in edge order, 0 for a pair without an edge)."""
+    dev = _device(rest, "rest")
+    _, V, _ = _skin_sizes(rest, None, None)
+    F = faces.shape[0] if faces.dim() == 2 else 0
+    _icp_tensor(faces, (F, 3), "faces")
+    _skin_slots(joints, weights, V)
+    B = int(n_bones)
+    n = C.c_int64()
+    _lib.check(_abi.amb_autorig_pair_scratch_ints(V, F, B, C.byref(n)), "amb_autorig_pair_scratch_ints")
+    scratch = torch.empty(n.value, dtype=torch.int32, device=rest.device)
+    P = B * (B - 1) // 2
+    count = torch.zeros(P, dtype=torch.int32, device=rest.device)
+    prior = torch.zeros(P, 3, dtype=torch.float64, device=rest.device)
+    _launch(_abi.amb_autorig_pair_stats, 16 if P else 0, _ptr(rest, torch.float64, "rest", dev), V,
+            _ptr(faces, torch.int32, "faces", dev), F, _ptr(joints, torch.int32, "joints", dev),
+            _ptr(weights, torch.float64, "weights", dev), B, _ptr(scratch, torch.int32, "scratch", dev),
+            _ptr(count, torch.int32, "pair_count", dev), _ptr(prior, torch.float64, "pair_prior", dev),
+            tag="autorig_pair_stats")
+    return count, prior
+
+
+def autorig_bone_weights(joints: torch.Tensor, weights: torch.Tensor, n_bones: int) -> torch.Tensor:
+    """-> totals (B) fp64: each bone's sum of used-slot weights, per 256-vertex tile then in tile order."""
+    dev = _device(weights, "weights")
+    V = weights.shape[0]
+    _skin_slots(joints, weights, V)
+    B = int(n_bones)
+    scratch = torch.empty(-(-V // 256) * B, dtype=torch.float64, device=weights.device)
+    totals = torch.empty(B, dtype=torch.float64, device=weights.device)
+    _launch(_abi.amb_autorig_bone_weights, 2, _ptr(joints, torch.int32, "joints", dev),
+            _ptr(weights, torch.float64, "weights", dev), V, B, _ptr(scratch, torch.float64, "scratch", dev),
+            _ptr(totals, torch.float64, "totals", dev))
+    return totals
+
+
+def autorig_joint_solve(transforms: torch.Tensor, centres: torch.Tensor, pair_count: torch.Tensor,
+                        pair_prior: torch.Tensor, lam: float) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per pair of bones of `transforms` (T, B, 12), the point both map alike, pulled towards its prior by `lam` ->
+    (pair_joint (P, 3) fp64, pair_cost (P) fp64 = the mean squared mismatch per frame)."""
+    dev = _device(transforms, "transforms")
+    T, B = transforms.shape[0], transforms.shape[1] if transforms.dim() == 3 else 0
+    _icp_tensor(transforms, (T, B, 12), "transforms")
+    _icp_tensor(centres, (B, 3), "centres")
+    P = B * (B - 1) // 2
+    _icp_tensor(pair_count, (P,), "pair_count")
+    _icp_tensor(pair_prior, (P, 3), "pair_prior")
+    if not lam > 0:
+        raise _lib.AmbError(f"lambda must be > 0, got {lam}")
+    lam_t = torch.full((1,), float(lam), dtype=torch.float64, device=transforms.device)
+    joint = torch.empty(P, 3, dtype=torch.float64, device=transforms.device)
+    cost = torch.empty(P, dtype=torch.float64, device=transforms.device)
+    _launch(_abi.amb_autorig_joint_solve, 1 if P else 0, _ptr(transforms, torch.float64, "transforms", dev), T, B,
+            _ptr(centres, torch.float64, "centres", dev), _ptr(pair_count, torch.int32, "pair_count", dev),
+            _ptr(pair_prior, torch.float64, "pair_prior", dev), _ptr(lam_t, torch.float64, "lambda", dev), _ptr(joint, torch.float64, "pair_joint", dev),
+            _ptr(cost, torch.float64, "pair_cost", dev), tag="autorig_joint_solve")
+    return joint, cost
+
+
+def autorig_slots(joints: torch.Tensor, weights: torch.Tensor, slot_bind: torch.Tensor, slot_weight: torch.Tensor) -> None:
+    """(V, 4) joints / weights -> the rig's (V, 8) slot_bind / slot_weight (in place), used slots first, then 0 / 0."""
+    dev = _device(weights, "weights")
+    V = weights.shape[0]
+    _skin_slots(joints, weights, V)
+    _icp_tensor(slot_bind, (V, 8), "slot_bind")
+    _icp_tensor(slot_weight, (V, 8), "slot_weight")
+    _launch(_abi.amb_autorig_slots, 1, _ptr(joints, torch.int32, "joints", dev), _ptr(weights, torch.float64, "weights", dev),
+            V, _ptr(slot_bind, torch.int32, "slot_bind", dev), _ptr(slot_weight, torch.float64, "slot_weight", dev))
+
+
+def autorig_list_scratch(n_vertices: int, n_joints: int, device) -> torch.Tensor:
+    """The int32 scratch `autorig_joint_lists` needs for these sizes."""
+    n = C.c_int64()
+    _lib.check(_abi.amb_autorig_list_scratch_ints(int(n_vertices), int(n_joints), C.byref(n)),
+               "amb_autorig_list_scratch_ints")
+    return torch.empty(n.value, dtype=torch.int32, device=device)
+
+
+def autorig_joint_lists(rig, subtree_end: torch.Tensor, lists: torch.Tensor, offsets: torch.Tensor,
+                        scratch: Optional[torch.Tensor] = None) -> None:
+    """Rebuild the per-joint vertex lists of `rig` (a `rig.RigTensors`, joints depth-first) from its slots: joint k's
+    vertices in ascending order, lists[offsets[k]:offsets[k + 1]] (in place on `lists` (capacity) and `offsets` (J + 1)
+    int32).  Entries past the capacity are dropped: the caller checks offsets[J] <= capacity."""
+    dev = _device(rig.slot_weight, "slot_weight")
+    V, J = rig.points.shape[0], subtree_end.shape[0]
+    _icp_tensor(rig.slot_bind, (V, 8), "slot_bind")
+    _icp_tensor(rig.slot_weight, (V, 8), "slot_weight")
+    _icp_tensor(offsets, (J + 1,), "offsets")
+    cap = _rig_list(lists)
+    if scratch is None:
+        scratch = autorig_list_scratch(V, J, rig.slot_weight.device)
+    _launch(_abi.amb_autorig_joint_lists, 3, _ptr(rig.bind_joint, torch.int32, "bind_joint", dev),
+            _ptr(rig.slot_bind, torch.int32, "slot_bind", dev), _ptr(rig.slot_weight, torch.float64, "slot_weight", dev), V,
+            _ptr(subtree_end, torch.int32, "subtree_end", dev), J, _ptr(scratch, torch.int32, "scratch", dev),
+            _ptr(lists, torch.int32, "lists", dev), cap, _ptr(offsets, torch.int32, "offsets", dev),
+            tag="autorig_joint_lists")
+
+
 # ---- background removal: RMBG-1.4's resampling, im2col, mask head and refinement (csrc/rmbg.cu) ------------------------------
 # Activations are fp32 NHWC feature maps held as 2-D (H * W, pixel stride) tensors with unit channel stride: a GEMM output
 # padded to 64 columns is read in place, its first C columns being the channels.

@@ -98,6 +98,16 @@ def _rotation_matrix(q) -> np.ndarray:
     return _node_matrix({"rotation": list(q)})[:3, :3]
 
 
+def subtree_ends(parent) -> np.ndarray:
+    """(J) int64: one past the last joint of each joint's subtree, for joints in a depth-first order (parent[k] < k)."""
+    parent = np.asarray(parent)
+    end = np.arange(1, len(parent) + 1)
+    for k in range(len(parent) - 1, -1, -1):
+        if parent[k] >= 0:
+            end[parent[k]] = max(end[parent[k]], end[k])
+    return end
+
+
 def rig_arrays(rig) -> RigArrays:
     """The host side of a fit: the joints in topological order, every bind and slot renumbered, and the per-joint vertex
     lists, each built once per fit."""
@@ -109,10 +119,7 @@ def rig_arrays(rig) -> RigArrays:
     parent = np.where(par >= 0, pos[np.maximum(par, 0)], -1)
     if (parent >= np.arange(J)).any():
         raise ValueError("rig.order is not a topological order of the joints")
-    end = np.arange(1, J + 1)
-    for k in range(J - 1, -1, -1):
-        if parent[k] >= 0:
-            end[parent[k]] = max(end[parent[k]], end[k])
+    end = subtree_ends(parent)
     if not all((parent[k + 1:end[k]] >= k).all() for k in range(J)):
         raise ValueError("rig.order is not a depth-first order of the joints")
     above = _xf12(np.asarray(rig.above)[order])
@@ -153,6 +160,20 @@ def rig_tensors(a: RigArrays, frames: int, device) -> RigTensors:
                       scratch=ops.rig_scratch(frames, len(a.points), device))
 
 
+def run_sweeps(t: RigTensors, parent, subtree_end, rot: torch.Tensor, trans: torch.Tensor, verts: torch.Tensor,
+               joint_lists: list, history: torch.Tensor) -> None:
+    """len(history) coordinate-descent sweeps of the state (rot, trans) in place: every joint in order takes its exact
+    rotation update over joint_lists[k], then a root its translation update; history[s] (T + 1) receives the error after
+    sweep s.  Everything is enqueued, with no host round trip."""
+    for s in range(history.shape[0]):
+        for k in range(len(parent)):
+            end = int(subtree_end[k])
+            ops.rig_rotation_update(t, rot, trans, verts, joint_lists[k], k, end)
+            if parent[k] < 0:
+                ops.rig_translation_update(t, rot, trans, verts, joint_lists[k], k, end)
+        ops.rig_error(t, rot, trans, verts, history[s])
+
+
 def fit_rig_animation(rig, vertices, sweeps: int = DEFAULT_SWEEPS, device: Optional[torch.device] = None) -> RigFit:
     """Fit the local joint rotations and root translations of `rig` (a `gltf.GltfRig`) to the (T, V, 3) animation
     `vertices` (in `load_glb`'s vertex order and frame) -> RigFit.  ValueError: a non-finite value, a shape that does not
@@ -178,13 +199,7 @@ def fit_rig_animation(rig, vertices, sweeps: int = DEFAULT_SWEEPS, device: Optio
         joint_lists = [lists[int(a.offsets[k]):int(a.offsets[k + 1])] for k in range(J)]
         history = torch.empty(sweeps + 1, T + 1, dtype=torch.float64, device=dev)
         ops.rig_error(t, rot, trans, verts, history[0])
-        for s in range(sweeps):
-            for k in range(J):
-                end = int(a.subtree_end[k])
-                ops.rig_rotation_update(t, rot, trans, verts, joint_lists[k], k, end)
-                if a.parent[k] < 0:
-                    ops.rig_translation_update(t, rot, trans, verts, joint_lists[k], k, end)
-            ops.rig_error(t, rot, trans, verts, history[s + 1])
+        run_sweeps(t, a.parent, a.subtree_end, rot, trans, verts, joint_lists, history[1:])
         frame_errors, max_error2 = ops.rig_error(t, rot, trans, verts)
         rot_pre, trans_pre = rot.cpu().numpy(), trans.cpu().numpy()
         hist = history[:, T].cpu().numpy().tolist()

@@ -527,6 +527,43 @@ int amb_rig_error(const int32_t* parent, int n_joints, const double* scale, cons
                   int64_t n_vertices, const int32_t* slot_bind, const double* slot_weight, double* scratch,
                   double* frame_errors, double* max_error2, amb_stream_t stream);
 
+/* ---- automatic rig: a joint hierarchy found from SSDR bones and refitted (csrc/autorig.cu; DESIGN.md §22) --------------
+ * actionmesh_b200/autorig.py drives the calls.  All arithmetic is fp64 with each operation rounded on its own, in the order
+ * DESIGN.md §22 states; no floating-point value is accumulated atomically.  Bones i < j of B (1 <= B <= min(V, 256)) form
+ * pair p = i (2B - i - 1) / 2 + (j - i - 1), P = B (B - 1) / 2 pairs in lexicographic order.  joints (V, 4) int32 and
+ * weights (V, 4) fp64 are skin_weight_update's layout, a slot being used when its weight is > 0.
+ *  autorig_pair_scratch_ints: the int32 scratch autorig_pair_stats needs (1 <= F <= 2^31 / 3 - 256).
+ *  autorig_pair_stats: every face edge (f_k, f_(k+1) mod 3) whose ends have different dominant bones (a vertex's used slot of
+ *    largest weight, ties to the earlier slot) counts for its pair: pair_count (P) int32 = the number of such edges,
+ *    pair_prior (P, 3) = the mean of their rest midpoints summed in edge order (0 without an edge).  P == 0 launches and
+ *    checks nothing else.
+ *  autorig_bone_weights: totals (B) = sum_v of bone b's used-slot weights, per 256-vertex tile then in tile order; scratch
+ *    holds ceil(V / 256) B doubles.
+ *  autorig_joint_solve: per pair, with D = R_i^t - R_j^t and d = t_j^t - t_i^t from transforms (T, B, 12), pair_joint (P, 3)
+ *    = argmin_c sum_t |D c - d|^2 + lambda T |c - m|^2 (m = the prior when pair_count > 0, else (c_i + c_j) / 2 from
+ *    centres (B, 3)), by Cholesky; pair_cost (P) = sum_t |D c - d|^2 / T.  lambda: one fp64 > 0 (device).
+ *  autorig_slots: (V, 4) joints / weights -> slot_bind (V, 8) int32 / slot_weight (V, 8), used slots first, then 0 / 0.
+ *  autorig_list_scratch_ints: the int32 scratch autorig_joint_lists needs (J V < 2^31 - 1).
+ *  autorig_joint_lists: for the rig layout of amb_rig_* (joints depth-first, subtree_end (J) int32), lists = joint k's
+ *    vertices (those whose used slots hold a bind of a joint in [k, subtree_end[k])) in ascending order, joint after joint,
+ *    and offsets (J + 1) int32 their starts then the total; entries past `capacity` are not written (the caller checks
+ *    offsets[J] <= capacity). */
+int amb_autorig_pair_scratch_ints(int64_t n_vertices, int64_t n_faces, int n_bones, int64_t* out_ints);
+int amb_autorig_pair_stats(const double* rest, int64_t n_vertices, const int32_t* faces, int64_t n_faces,
+                           const int32_t* joints, const double* weights, int n_bones, int32_t* scratch, int32_t* pair_count,
+                           double* pair_prior, amb_stream_t stream);
+int amb_autorig_bone_weights(const int32_t* joints, const double* weights, int64_t n_vertices, int n_bones, double* scratch,
+                             double* totals, amb_stream_t stream);
+int amb_autorig_joint_solve(const double* transforms, int frames, int n_bones, const double* centres,
+                            const int32_t* pair_count, const double* pair_prior, const double* lambda, double* pair_joint,
+                            double* pair_cost, amb_stream_t stream);
+int amb_autorig_slots(const int32_t* joints, const double* weights, int64_t n_vertices, int32_t* slot_bind,
+                      double* slot_weight, amb_stream_t stream);
+int amb_autorig_list_scratch_ints(int64_t n_vertices, int n_joints, int64_t* out_ints);
+int amb_autorig_joint_lists(const int32_t* bind_joint, const int32_t* slot_bind, const double* slot_weight,
+                            int64_t n_vertices, const int32_t* subtree_end, int n_joints, int32_t* scratch, int32_t* lists,
+                            int64_t capacity, int32_t* offsets, amb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
